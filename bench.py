@@ -29,20 +29,24 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOAD = dict(R=3, V=2, L=2)           # BASELINE configs[1] = vsr-revisited/paper/VSR.cfg
-TABLE_CAP = 1 << int(os.environ.get("VSR_BENCH_TABLE_LOG2", "32"))  # 2^32 slots * 16 B = 64 GiB over all GPUs (1.17e9 states -> load 0.27: measured 10 %
-                                                                     # less kernel time than 2^31, profiles/round2_expand_kernel.md) + 8 B of trace record per slot
+# 2^31 slots * 16 B = 32 GiB of seen-set (1.17e9 states -> load 0.55) + 7 B of trace record per slot + two frontiers of
+# 144 M states of 48 B: 59 GiB, what an 80 GB H100 holds with room to spare (2^32 slots would not fit beside the trace)
+TABLE_CAP = 1 << int(os.environ.get("VSR_BENCH_TABLE_LOG2", "31"))
 FRONTIER_CAP = 140_000_000               # widest level: 120,193,500 states
 EXPECT = dict(distinct=1173992337, generated=3129587684, depth=47, violation_level=28)
 # a configuration BOTH arms finish: (R=3, V=2, L=1) WITHOUT SYMMETRY, complete = 697,364 distinct states, depth 30 - totals pinned to
 # the spec's text (tests/golden/spec_text_results.json) - the same-config comparison beside the bounded cfg2 sample of the CPU arm
 SMALL = dict(R=3, V=2, L=1, symmetry=0, distinct=697364, generated=1831657, depth=30)
 # BASELINE configs[2]/[4]: README constants to the first AcknowledgedWriteNotLost violation, at every GPU count
-# Sizes per GPU count (level 24 alone is 1.345e9 states of 64 B; 3.17e9 seen-set entries + trace records): one GPU holds the seen-set,
-# the trace and 2 x 560 M frontier states in HBM and lets each frontier buffer continue with 850 M states in pinned host memory (spill)
+# Sizes per GPU count (level 24 alone is 1.345e9 states of 64 B; 3.17e9 seen-set entries + trace records at 23 B per slot), each
+# within an 80 GB H100: 2 GPUs hold 2e9 slots (46 GB) and 2 x 150 M frontier states (19 GB) each and let every frontier buffer
+# continue with 560 M states in pinned host memory (spill); 4 GPUs 1e9 slots and 2 x 300 M states + 100 M in host memory;
+# 8 GPUs 1.07e9 slots and 2 x 200 M states.  One GPU cannot hold it: the seen-set and the trace alone need 83 GB.
 CFG3 = dict(R=3, V=3, L=3, violation_level=24, distinct=3166753191,
-            table_total={1: 4_000_000_000, 2: 4_400_000_000, 4: 1 << 33, 8: 1 << 33},
-            frontier_total={1: 560_000_000, 2: 1_500_000_000, 4: 1_600_000_000, 8: 1_600_000_000},
-            frontier_host={1: 850_000_000, 2: 0, 4: 0, 8: 0})
+            table_total={2: 4_000_000_000, 4: 4_000_000_000, 8: 1 << 33},
+            frontier_total={2: 300_000_000, 4: 1_200_000_000, 8: 1_600_000_000},
+            frontier_host={2: 560_000_000, 4: 100_000_000, 8: 0})
+DUMP_WALK = 4096                         # --dump-outputs: states of the seeded walk looked up in the seen-set
 
 
 def peaks():
@@ -50,7 +54,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback: H100 SXM data sheet, 3.35 TB/s (not measured)"
 
 
 class ClockSampler:
@@ -150,14 +154,14 @@ def small_complete_cpu(cores):
 
 
 def try_tlc(seconds):
-    """BASELINE.md: if a JVM and tla2tools.jar ever appear on the box ($TLA2TOOLS_JAR) together with the spec ($VSR_TLA, or the
-    reference checkout), run the REAL reference — TLC — on the same config for a bounded time and return its rate.  In this
-    image there is no java, so this returns None and the CPU restatement stands in."""
+    """BASELINE.md: if a JVM and tla2tools.jar ever appear on the machine ($TLA2TOOLS_JAR) together with the spec ($VSR_TLA), run
+    the REAL reference — TLC — on the same config for a bounded time and return its rate.  Without them this returns None and
+    the CPU restatement stands in."""
     import re
     import shutil
     import tempfile
     jar, java = os.environ.get("TLA2TOOLS_JAR"), shutil.which("java")
-    tla = os.environ.get("VSR_TLA", "/root/reference/vsr-revisited/paper/VSR.tla")
+    tla = os.environ.get("VSR_TLA", "")
     if not (jar and java and os.path.exists(jar) and os.path.exists(tla)):
         return None
     import _pkg
@@ -243,6 +247,12 @@ def host_memory_available():
     return avail
 
 
+def pinning_fits(pinned_per_rank, node_ranks, avail):
+    """may the node_ranks ranks of one machine each pin pinned_per_rank bytes of host memory, with avail bytes available to the
+    job (host_memory_available(), read before any of them has pinned)?  Pinned pages cannot be swapped: keep 40 % free."""
+    return avail is not None and pinned_per_rank * node_ranks <= 0.6 * avail
+
+
 def golden_depths(pkg, mc, eng, torch, tdist, world, dev, rank):
     """BFS depth at which each state of the reference's published 24-state counterexample (tests/golden/
     state_transfer_trace.json, generated from state_transfer_violation_trace.txt) was first seen; 0 = not in the explored set"""
@@ -268,10 +278,16 @@ def cfg3_first_violation(pkg, vdist, torch, tdist, group, rank, world, local, de
     mc = pkg.ModelChecker.from_constants(CFG3["R"], CFG3["V"], CFG3["L"])
     pinned = 2 * CFG3["frontier_host"][world] * mc.state_bytes
     if pinned:
+        # every rank on this machine pins its own share: the decision is on their sum, read before any of them has pinned,
+        # and taken together (one rank that went ahead alone would wait for the others forever)
+        node_ranks = int(os.environ.get("LOCAL_WORLD_SIZE", world))
         avail = host_memory_available()
-        if avail is None or pinned > 0.6 * avail:
-            return {"skipped": "needs %.0f GB of pinned host memory for the frontier spill; %s available to this job"
-                               % (pinned / 1e9, "unknown" if avail is None else "%.0f GB" % (avail / 1e9))}
+        ok = torch.tensor([int(pinning_fits(pinned, node_ranks, avail))], dtype=torch.int32, device=dev)
+        if world > 1:
+            tdist.all_reduce(ok, op=tdist.ReduceOp.MIN)
+        if not int(ok.item()):
+            return {"skipped": "needs %.0f GB of pinned host memory for the frontier spill (%d ranks on this machine); %s available to this job"
+                               % (pinned * node_ranks / 1e9, node_ranks, "unknown" if avail is None else "%.0f GB" % (avail / 1e9))}
     table_cap = CFG3["table_total"][world] // world
     frontier_cap = CFG3["frontier_total"][world] // world
     barrier()
@@ -301,6 +317,35 @@ def cfg3_first_violation(pkg, vdist, torch, tdist, group, rank, world, local, de
     return out
 
 
+def dump_outputs(out_dir, mc, eng, res, torch, tdist, world, dev, rank):
+    """What the last timed BFS computed, as .npy files that two builds can be compared by: the per-depth state and successor
+    counts, the totals (distinct, generated, depth, queue, first violating depth, complete, VIEW ties, fingerprint collisions),
+    and the depth at which the seen-set holds each state of a seeded random walk of Next from Init (a fixed
+    sample of the explored set; 0 = not in it).  The walk uses the host's Next, so it is the same whatever the GPU computed."""
+    import random
+    import numpy as np
+    rng = random.Random(20240601)
+    walk, s = [], mc.init_state()
+    while len(walk) < DUMP_WALK:
+        walk.append(s)
+        succ = mc.successors(s)
+        s = rng.choice(succ)[0] if succ else mc.init_state()
+    depths = []
+    for s in walk:
+        lvl, owner = eng.lookup(s)
+        depths.append(lvl if owner == rank else 0)
+    t = torch.tensor(depths, dtype=torch.int64, device=dev)
+    if world > 1:
+        tdist.all_reduce(t, op=tdist.ReduceOp.MAX)
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    totals = [res.distinct, res.generated, res.depth, res.queue, res.violation_level, int(res.complete), res.h2_ties, res.fp_collisions]
+    for name, a in (("level_sizes", res.level_sizes), ("level_generated", res.level_generated), ("walk_depths", t.cpu().tolist()),
+                    ("totals", totals)):
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -310,9 +355,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=15.0)
     ap.add_argument("--no-cfg3", action="store_true", help="N >= 2: skip the README-constants first-violation block (BASELINE configs[2]/[4])")
-    ap.add_argument("--cfg3-one-gpu", action="store_true",
-                    help="N = 1: run that block too: 3.17e9 states on ONE GPU with the frontier spilling into 109 GB of pinned host memory "
-                         "(off by default: a box that is a slice of a machine may not have that much)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last one computed to DIR/<name>.npy")
     ap.add_argument("--no-e2e", action="store_true", help="profiling runs: skip the end-to-end legs")
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "staged"],
                     help="N > 1: p2p = the kernel stores remote successors into the owner's inbox over NVLink, C++ level loop (default); "
@@ -394,6 +437,8 @@ def main():
     wall = float(t[0])
     clocks = sampler.stop() if rank == 0 else None
     st = eng.stats()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, mc, eng, res, torch, tdist, world, dev, rank)
 
     ok = (res.distinct == EXPECT["distinct"] and res.generated == EXPECT["generated"] and res.depth == EXPECT["depth"] and
           res.violation_level == EXPECT["violation_level"] and res.complete)
@@ -405,13 +450,6 @@ def main():
     kern_s = kernel_ms / 1e3                 # sum over levels of the slowest rank's kernel time, all timed steps
     achieved = (res.distinct / world) * args.steps * b_alg / kern_s / 1e9
     peak, peak_src = peaks()
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "round2_traffic.json")  # ncu --set full dram bytes of one wide level of THIS configuration
-    if os.path.exists(tpath):
-        try:
-            traffic = json.load(open(tpath))
-        except ValueError:
-            traffic = None
 
     probe = None
     eng.close()
@@ -456,7 +494,7 @@ def main():
     e2e_s = sorted(e2e_runs)[1] if e2e_runs else None
 
     cfg3 = None
-    if (world > 1 and not args.no_cfg3 and not staged) or (world == 1 and args.cfg3_one_gpu):
+    if world > 1 and not args.no_cfg3 and not staged:
         torch.cuda.empty_cache()
         try:
             cfg3 = cfg3_first_violation(pkg, vdist, torch, tdist, group, rank, world, local, dev, barrier)
@@ -491,7 +529,7 @@ def main():
                        "results_match_expected": bool(ok),
                        "oracle_coverage": "GPU == CPU oracle as SETS for complete spaces <= 697k states and to a bounded depth of this config "
                                           "(tests/test_gpu_parity.py); the full-size totals are checked against the numbers every earlier run "
-                                          "and every GPU count reproduced, not against an oracle run (the oracle does 4e5 states/s)",
+                                          "and every GPU count reproduced, not against an oracle run (too large for the CPU oracle: its rate is cpu_baseline)",
                        "timing": "wall clock bracketed by barrier+synchronize, max over ranks; "
                        "device time between CUDA events on the launch stream = %.3f s" % (dev_ms / 1e3)},
             "gpu_launches": launches0,
@@ -504,8 +542,6 @@ def main():
             "level_ms_last_step": [round(x, 4) for x in levels_ms[-1]] if levels_ms else [],
             "level_sizes": [int(x) for x in res.level_sizes],
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic.get("dram_bytes_per_launch") if traffic else None,
-                         "traffic_note": (traffic.get("note") if traffic else "no ncu capture of this configuration committed yet (profiles/round2_traffic.json)"),
                          "peak_source": peak_src, "bytes_per_state": b_alg, "g": g,
                          "widest_level": {"depth": wide + 1, "ms": levels_ms[-1][wide] if levels_ms and levels_ms[-1] else None,
                                           "states_expanded": int(res.level_sizes[wide]) if res.level_sizes else None},

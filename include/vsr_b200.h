@@ -1,5 +1,5 @@
 /*
- * vsr_b200.h — C ABI of the B200-native explicit-state model checker for
+ * vsr_b200.h — C ABI of the H100-native explicit-state model checker for
  * vsr-revisited/paper/VSR.tla (reference: Vanlightly/vsr-tlaplus @ 7566e8af).
  *
  * What this replaces.  The reference has no plugin/operator ABI: TLA+ has no FFI and the path

@@ -3,7 +3,7 @@ vsr-revisited/paper/VSR.tla of the reference is written in.
 
 Why: the C++ oracle (vsr_oracle.cpp) is my restatement of the spec; TLC — the tool that gives the spec its meaning — is
 not in this image (no JVM).  This module executes the reference's OWN SOURCE TEXT: it parses VSR.tla as it lies under
-/root/reference and enumerates Init and the successors of a state the way TLC does (conjuncts left to right, x' = e
+the reference (Vanlightly/vsr-tlaplus) and enumerates Init and the successors of a state the way TLC does (conjuncts left to right, x' = e
 assigns the first time and tests afterwards, \\E and \\/ branch, UNCHANGED copies, operator definitions are expanded).
 tests/test_spec_text.py compares, state by state, the successor sets it derives from the text with the oracle's, and
 whole small state spaces level by level.  It pins the oracle to the spec's text rather than to my reading of it.
@@ -12,7 +12,7 @@ Scope: exactly the constructs VSR.tla uses (junction lists by column, \\E/\\A/CH
 with @ and nested paths, sets, sequences, Quantify/LAMBDA, Permutations, model values).  Not a general TLA+ tool, no
 liveness, no TLC value ORDER: CHOOSE takes the first candidate in this module's own order and REPORTS when more than one
 candidate satisfied the predicate (see Evaluator.choose_log), so a caller can tell whether a result depended on the pick.
-Nothing here is imported by the product; the GPU box never runs it (it needs /root/reference).
+Nothing here is imported by the product; the tests replay what it answered on the spec's text (tests/spec_text.py).
 """
 import re
 from itertools import permutations, product

@@ -1,6 +1,6 @@
 /*
  * tlc_text.cpp — TLC "dumpTrace tlc" value text: printer and parser (oracle side; test
- * infrastructure only).  The format is the one of /root/reference/state_transfer_violation_trace.txt:
+ * infrastructure only).  The format is the one of tests/golden/state_transfer_violation_trace.txt.gz:
  * variables alphabetical, functions over 1..n as <<...>>, other functions as (k :> v @@ ...),
  * records [f |-> v, ...] with fields in first-interned order, sets {...}, intervals a..b.
  */

@@ -2,7 +2,7 @@
  * vsr_oracle.cpp — semantics of VSR.tla restated on the CPU (see vsr_oracle.h header comment:
  * test infrastructure only; pinned to state_transfer_violation_trace.txt and, through oracle/tla_eval.py,
  * to the text of VSR.tla itself; TLC's fingerprint values and the totals of the big configurations unpinned).
- * Every function cites the lines of /root/reference/vsr-revisited/paper/VSR.tla it follows.
+ * Every function cites the lines of the reference's vsr-revisited/paper/VSR.tla it follows.
  */
 #include "vsr_oracle.h"
 

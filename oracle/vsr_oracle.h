@@ -12,7 +12,7 @@
  * AcknowledgedWriteNotLost, and print_state() reproduces the file's text byte for byte apart from
  * `location` strings and three variables the file predates).
  * Second pin: the reference's own SOURCE TEXT.  oracle/tla_eval.py parses VSR.tla as it lies under
- * /root/reference and enumerates Init/Next the way TLC does; tests/test_spec_text.py compares it with
+ * the reference (Vanlightly/vsr-tlaplus) and enumerates Init/Next the way TLC does; tests/test_spec_text.py compares it with
  * this file — complete state spaces level by level (cfg1 = BASELINE configs[0]: 76 distinct / 100
  * generated / depth 14, and eight more up to 697,364 states), successor sets state by state along the golden trace,
  * random walks on cfg2/cfg3/cfg4 constants, the recovery actions with RestartEmptyLimit 1 and 2, both

@@ -7,14 +7,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-REFERENCE = "/root/reference"
-REF_TLA = os.path.join(REFERENCE, "vsr-revisited/paper/VSR.tla")
-REF_CFG = os.path.join(REFERENCE, "vsr-revisited/paper/VSR.cfg")
-REF_TRACE = os.path.join(REFERENCE, "state_transfer_violation_trace.txt")
+# the reference's published counterexample (TLC `dumpTrace tlc` text of VSR.tla, README constants), gzip-compressed
+REF_TRACE = os.path.join(ROOT, "tests", "golden", "state_transfer_violation_trace.txt.gz")
+# the reference's shipped TLC configuration, vsr-revisited/paper/VSR.cfg
+REF_CFG = os.path.join(ROOT, "tests", "golden", "VSR.cfg")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -27,10 +27,3 @@ def pkg():
         __graft_entry__.build()
     return _pkg.load()
 
-
-@pytest.fixture(scope="session")
-def have_reference():
-    return os.path.exists(REF_TLA)
-
-
-needs_reference = pytest.mark.skipif(not os.path.exists(REF_TLA), reason="/root/reference is not mounted here")

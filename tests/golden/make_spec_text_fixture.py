@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generates tests/golden/spec_text_results.json: what oracle/tla_eval.py derives from the TEXT of the reference's
-vsr-revisited/paper/VSR.tla (read from /root/reference — this script only runs where the reference is mounted).
+vsr-revisited/paper/VSR.tla (named by VSR_SPEC_TLA: this script only runs where a checkout of the reference is at hand).
 
   state_spaces   level sizes / successors generated per level / totals of breadth-first searches run by the text
                  evaluator (SYMMETRY off, VIEW on), complete for the small configurations, depth-bounded for bigger ones
@@ -10,9 +10,9 @@ vsr-revisited/paper/VSR.tla (read from /root/reference — this script only runs
                  behaviour of the text (action names of profiles/cfg2_counterexample)
 
 tests/test_spec_text.py::test_oracle_equals_the_committed_spec_text_results checks the oracle against `state_spaces`
-on every machine (the GPU box has no /root/reference).
+on every machine.
 
-    python tests/golden/make_spec_text_fixture.py                          # everything (about 20 minutes)
+    VSR_SPEC_TLA=<reference>/vsr-revisited/paper/VSR.tla python tests/golden/make_spec_text_fixture.py   # everything (about 20 minutes)
     python tests/golden/make_spec_text_fixture.py --add-space R V L DEPTH  # one more state space (DEPTH 0 = complete)
 """
 import base64

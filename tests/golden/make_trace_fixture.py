@@ -1,15 +1,16 @@
 #!/usr/bin/env python
 """Generates tests/golden/state_transfer_trace.json from the reference's only golden vector,
-/root/reference/state_transfer_violation_trace.txt (24 states, TLC `dumpTrace tlc` text).
+state_transfer_violation_trace.txt (24 states, TLC `dumpTrace tlc` text; a gzip-compressed copy is in tests/golden/).
 
 The reference file is parsed with the oracle's TLC-value parser; each state is stored as the raw bytes
 of a VsrFlatState (include/vsr_flat.h; zlib + base64, the struct is mostly zeros) next to its action
-name.  The fixture travels to the GPU box, where /root/reference does not exist.
+name.
 
     python tests/golden/make_trace_fixture.py
 """
 import base64
 import ctypes as C
+import gzip
 import json
 import os
 import sys
@@ -23,13 +24,13 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import _pkg  # noqa: E402
 import orc  # noqa: E402
 
-SRC = "/root/reference/state_transfer_violation_trace.txt"
+SRC = os.path.join(HERE, "state_transfer_violation_trace.txt.gz")
 
 
 def main():
     pkg = _pkg.load()
     Flat = pkg.checker.VsrFlatState
-    text = open(SRC, "rb").read()
+    text = gzip.open(SRC).read()
     cap = 64
     flats = (Flat * cap)()
     acts = (C.c_int * cap)()

@@ -1,7 +1,15 @@
 """Helpers for tests/test_spec_text.py: the reference's VSR.tla executed by oracle/tla_eval.py, side by side with the
-C++ oracle.  States travel between the two as text: the oracle prints a state (TLC value syntax), tla_eval parses it."""
+C++ oracle.  States travel between the two as text: the oracle prints a state (TLC value syntax), tla_eval parses it.
+
+The spec's text is not part of this repository.  What the text evaluator answered is stored in tests/golden/
+spec_text_answers.json, in the order the tests ask; the tests compare the oracle and the product with those answers.
+With VSR_SPEC_TLA naming the reference's VSR.tla, the evaluator runs on the text instead and the answers are recorded
+again (tests/golden/make_spec_text_answers.py)."""
+import atexit
 import collections
 import ctypes as C
+import hashlib
+import json
 import os
 import random
 import sys
@@ -12,7 +20,8 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import tla_eval as T  # noqa: E402
 import orc  # noqa: E402
 
-SPEC = "/root/reference/vsr-revisited/paper/VSR.tla"
+SPEC = os.environ.get("VSR_SPEC_TLA")
+ANSWERS = os.path.join(ROOT, "tests", "golden", "spec_text_answers.json")
 ACTIONS = ["Initial predicate", "TimerSendSVC", "ReceiveHigherSVC", "ReceiveMatchingSVC", "SendDVC", "ReceiveHigherDVC",
            "ReceiveMatchingDVC", "SendSV", "ReceiveSV", "ReceiveClientRequest", "ReceivePrepareMsg", "ReceivePrepareOkMsg",
            "ExecuteOp", "SendGetState", "ReceiveGetState", "ReceiveNewState", "RestartEmpty", "ReceivesRecoveryMsg",
@@ -20,7 +29,58 @@ ACTIONS = ["Initial predicate", "TimerSendSVC", "ReceiveHigherSVC", "ReceiveMatc
 
 
 def evaluator(R, V, L, restart=0):
-    return T.load_vsr(SPEC, R, 1, ["v%d" % (i + 1) for i in range(V)], L, restart)
+    """the text evaluator, or None when only the recorded answers are available"""
+    return T.load_vsr(SPEC, R, 1, ["v%d" % (i + 1) for i in range(V)], L, restart) if SPEC else None
+
+
+_recorded = None
+
+
+class Answers:
+    """The text's answers to one test, in the order it asks.  value(fn): with the spec's text, fn() is computed, stored and
+    returned; without it, the stored answer is returned.  Answers are JSON values (lists, not tuples)."""
+
+    def __init__(self, name):
+        global _recorded
+        self.name = name
+        if SPEC:
+            self.seq = []
+            if name is None:  # a comparison no test replays (tests/golden/make_spec_text_fixture.py's sweep)
+                return
+            if _recorded is None:
+                _recorded = {}
+                atexit.register(_write_answers)
+            _recorded[name] = self.seq
+        else:
+            with open(ANSWERS) as f:
+                self.seq = json.load(f)[name]
+        self.i = 0
+
+    def value(self, fn):
+        if SPEC:
+            v = json.loads(json.dumps(fn()))
+            self.seq.append(v)
+            return v
+        assert self.i < len(self.seq), "%s asks more of the text than was recorded" % self.name
+        self.i += 1
+        return self.seq[self.i - 1]
+
+
+def _write_answers():
+    old = {}
+    if os.path.exists(ANSWERS):
+        with open(ANSWERS) as f:
+            old = json.load(f)
+    old.update(_recorded)
+    with open(ANSWERS, "w") as f:
+        f.write("{\n" + ",\n".join(json.dumps(k) + ":" + json.dumps(old[k], separators=(",", ":")) for k in sorted(old)) + "\n}\n")
+
+
+def digest(items):
+    """a multiset of values (tla_eval values, in tuples) as a short hash: the order of tla_eval.vkey, not of printing"""
+    def key(x):
+        return tuple(key(y) for y in x) if isinstance(x, tuple) else T.vkey(x)
+    return hashlib.sha1(repr(sorted(key(x) for x in items)).encode()).hexdigest()[:12]
 
 
 def to_py(q, flat):
@@ -30,9 +90,10 @@ def to_py(q, flat):
 class Pair:
     """one configuration: the text evaluator and the oracle (symmetry off: literal successors on both sides)"""
 
-    def __init__(self, pkg, R, V, L, restart=0):
+    def __init__(self, pkg, R, V, L, restart=0, name=None):
         self.Flat = pkg.checker.VsrFlatState
         self.ev = evaluator(R, V, L, restart)
+        self.text = Answers(name)
         self.q = orc.params(R, V, L, symmetry=False, restart=restart)
         self.q_awem = orc.params(R, V, L, symmetry=False, invariant=2, restart=restart)
         self.stats = collections.Counter()
@@ -56,6 +117,16 @@ class Pair:
         st = to_py(self.q, flat)
         osucc = self.oracle_successors(flat)
         want = collections.Counter((a, T.Fn(to_py(self.q, f))) for a, f in osucc)
+        text = self.text.value(lambda: self._text_answer(st, want))
+        assert text[0] == digest(want.elements()), "successors differ from the text's\nstate: %s" % {k: T.fmt(v) for k, v in st.items()}
+        for a, _ in osucc:
+            self.stats[a] += 1
+        assert text[1] == bool(orc.lib().orc_invariant_flat(self.q, C.byref(flat)))
+        assert text[2] == bool(orc.lib().orc_invariant_flat(self.q_awem, C.byref(flat)))
+        return osucc
+
+    def _text_answer(self, st, want):
+        """[digest of the text's successors, AcknowledgedWriteNotLost, AcknowledgedWritesExistOnMajority] of one state"""
         pick, got = 0, None
         while True:
             self.ev.choose_pick, self.ev.choose_log = pick, []
@@ -72,11 +143,8 @@ class Pair:
             only_orc = [(a, T.fmt(s)) for (a, s) in (want - got)]
             raise AssertionError("successors differ\nstate: %s\nonly from the text: %s\nonly from the oracle: %s" %
                                  ({k: T.fmt(v) for k, v in st.items()}, only_text[:3], only_orc[:3]))
-        for a, _ in osucc:
-            self.stats[a] += 1
-        assert self.ev.holds("AcknowledgedWriteNotLost", st) == bool(orc.lib().orc_invariant_flat(self.q, C.byref(flat)))
-        assert self.ev.holds("AcknowledgedWritesExistOnMajority", st) == bool(orc.lib().orc_invariant_flat(self.q_awem, C.byref(flat)))
-        return osucc
+        return [digest(got.elements()), bool(self.ev.holds("AcknowledgedWriteNotLost", st)),
+                bool(self.ev.holds("AcknowledgedWritesExistOnMajority", st))]
 
     def walk(self, flat, steps, rng, prefer=()):
         """compare along a random walk; `prefer` = actions taken whenever enabled (to reach rare neighbourhoods)"""

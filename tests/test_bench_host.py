@@ -1,5 +1,5 @@
-"""Host-side checks of bench.py that need no GPU: the driver runs bench.py only at round end on the GPU box, so a misspelt
-name there would cost the round's measurement."""
+"""Host-side checks of bench.py that need no GPU: bench.py runs only on a GPU machine, so a misspelt
+name there would cost a whole measurement run."""
 import builtins
 import os
 import symtable
@@ -62,14 +62,28 @@ def test_level_reduce_on_one_rank_is_the_identity():
     assert b._reduce_level([1, 2], [3], [4, 5]) == ([1, 2], [3], [4, 5])
 
 
-def test_one_gpu_readme_block_is_guarded_by_the_hosts_memory():
-    """bench.py pins 109 GB of host memory for the README constants on ONE GPU only when the job may have them (a box that is a
-    slice of a machine kills a job that pins past its cgroup limit instead of returning an error): the guard reads MemAvailable
-    and the cgroup limit, and the sizes of every GPU count are there"""
+def test_readme_block_is_guarded_by_the_hosts_memory():
+    """bench.py pins host memory for the README constants' frontier spill only when the job may have it (a box that is a slice
+    of a machine kills a job that pins past its cgroup limit instead of returning an error): the guard reads MemAvailable and
+    the cgroup limit and weighs the pinning of ALL ranks on the machine; the sizes of every GPU count are there and fit an
+    80 GB H100"""
     import bench
     avail = bench.host_memory_available()
     assert avail is None or 0 < avail < 1 << 50
-    for world in (1, 2, 4, 8):
+    state_bytes = 64  # Layout<3,3,4>
+    for world in (2, 4, 8):
         assert bench.CFG3["table_total"][world] // world * 7 // 8 >= bench.CFG3["distinct"] // world  # the seen-set's 7/8 load limit
         per_gpu = bench.CFG3["frontier_total"][world] // world + bench.CFG3["frontier_host"][world]
         assert per_gpu * world >= 1_344_894_424  # depth 24 of the README constants (profiles/cfg3_counterexample)
+        hbm = bench.CFG3["table_total"][world] // world * 23 + 2 * bench.CFG3["frontier_total"][world] // world * state_bytes
+        assert hbm < 72e9  # seen-set (16 B) + trace (7 B) per slot and two frontiers of 64 B states, with room for the inboxes
+        pinned = 2 * bench.CFG3["frontier_host"][world] * state_bytes  # per rank
+        if pinned:
+            # a share that one rank alone could pin is refused when all ranks of the machine together exceed the limit
+            assert bench.pinning_fits(pinned, 1, pinned / 0.6)
+            assert not bench.pinning_fits(pinned, world, pinned * world / 0.6 - 1)
+            assert bench.pinning_fits(pinned, world, pinned * world / 0.6 + 1)
+    # N = 2: 2 x 71.7 GB pinned on one machine; a job with 200 GB available must skip the block, not pin 143 GB
+    pinned2 = 2 * bench.CFG3["frontier_host"][2] * state_bytes
+    assert not bench.pinning_fits(pinned2, 2, 200e9) and bench.pinning_fits(pinned2, 2, 240e9)
+    assert not bench.pinning_fits(1, 1, None)

@@ -297,7 +297,7 @@ def test_shipped_cfg_full_size_properties(pkg):
       * the bounded-depth prefix agrees with the oracle-verified level sizes of test_bounded_depth_matches_oracle."""
     mc = pkg.ModelChecker.from_cfg_text(pkg.cfg_text(3, ["v1", "v2"], 2))
     a = mc.check(stop_on_violation=False, table_capacity=1 << 31, frontier_capacity=130_000_000)
-    b = mc.check(stop_on_violation=False, table_capacity=1 << 32, frontier_capacity=125_000_000, keep_trace=False)
+    b = mc.check(stop_on_violation=False, table_capacity=3_000_000_000, frontier_capacity=125_000_000, keep_trace=False)
     for r in (a, b):
         assert r.complete and r.error_code == 0 and r.queue == 0
         assert r.distinct == sum(r.level_sizes) == 1173992337

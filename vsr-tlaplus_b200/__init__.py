@@ -1,7 +1,7 @@
-"""vsr-tlaplus_b200 — B200-native explicit-state model checker for vsr-revisited/paper/VSR.tla.
+"""vsr-tlaplus_b200 — H100-native explicit-state model checker for vsr-revisited/paper/VSR.tla.
 
 The product is the C-ABI shared library ``libvsr_b200.so`` (include/vsr_b200.h): hand-written CUDA
-(sm_100a) BFS wavefront + a thin C++ host.  This package is only the Python mirror of TLC's
+(sm_90a) BFS wavefront + a thin C++ host.  This package is only the Python mirror of TLC's
 command-line surface for that one path (``ModelChecker`` ~ ``tlc2.TLC -config VSR.cfg VSR.tla``) and
 the multi-GPU pump (``dist``), which uses torch.distributed for the all-to-all plumbing.
 

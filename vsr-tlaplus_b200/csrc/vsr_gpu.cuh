@@ -1,5 +1,5 @@
 /*
- * vsr_gpu.cuh — device side of the BFS wavefront (sm_100a).
+ * vsr_gpu.cuh — device side of the BFS wavefront (sm_90a).
  *
  * One launch of expand_kernel<L> = TLC's worker loop (SURVEY §3.1 / §8a stages E1-E9) over one BFS
  * level of packed VSR.tla states:
@@ -21,7 +21,6 @@
  * prefix sums, one shared atomic per warp and action group, one barrier).  APPLY: warps take batches of 32 pairs of ONE
  * action and apply them one per lane — the successor is built in a rotated shared-memory row, read once into registers,
  * fingerprinted, probed, inserted — so the expensive part runs with full lanes and without divergence between actions.
- * See profiles/round1_expand_kernel.md for the measurements that led here.
  */
 #ifndef VSR_GPU_CUH
 #define VSR_GPU_CUH
@@ -167,9 +166,10 @@ __device__ __forceinline__ uint64_t make_meta(int level, uint32_t auxkey, uint32
 }
 
 /* lock-free insert-if-absent over 16-byte entries {fp, meta}.  A probe reads one BUCKET of VSR_BUCKET consecutive entries
-   (1: one 128-bit load; 2: one 256-bit load = a whole 32-byte sector; 4: two 256-bit loads issued together) and walks to
+   (1: one 128-bit load; 2: a whole 32-byte sector, read by ld256_cg as two 128-bit loads issued back to back — sm_90 has no
+   256-bit load; 4: two such sectors, all four loads issued together) and walks to
    the next bucket only when every slot of this one holds another state: the kernel is bound by the LATENCY of dependent
-   probes (profiles/round2_expand_kernel.md), so a wider first probe is paid for in bandwidth the kernel does not use.
+   probes, so a wider first probe is paid for in bandwidth the kernel does not use.
    Slots of a bucket fill in order (no deletions), so a lookup may stop at the first empty slot.  The bucket's entries
    are loaded by the caller as early as the fingerprint is known so that the HBM round trip overlaps the rest of the
    successor's work. */
@@ -178,7 +178,10 @@ __device__ __forceinline__ uint64_t make_meta(int level, uint32_t auxkey, uint32
 #endif
 struct Probe { uint64_t e[2 * VSR_BUCKET]; };
 __device__ __forceinline__ void ld256_cg(const uint64_t* p, uint64_t& a, uint64_t& b, uint64_t& c, uint64_t& d) {
-    asm volatile("ld.global.cg.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p) : "memory");
+    /* one 32-byte sector.  sm_90 has no 256-bit load: two 128-bit loads of the same sector, issued back to back so that
+       both are in flight together and cost one HBM round trip */
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%4];\n\tld.global.cg.v2.u64 {%2, %3}, [%4+16];"
+                 : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p) : "memory");
 }
 __device__ __forceinline__ unsigned long long table_home(unsigned long long cap, uint64_t fp) {
     /* bucket = floor(hash * nbuckets / 2^64): any capacity, no division.  The hash is the fingerprint times an odd constant
@@ -296,10 +299,9 @@ template <class L, int WARPS> struct BlockSmemT {
     WarpStage<L> w[WARPS];
 };
 /* Block shape.  ONE block of up to 32 warps per SM when its shared memory fits (227 KB), else two blocks of 16 / 12 / 8 warps
-   (2 x <= 113 KB).  Measured on the shipped VSR.cfg (profiles/round2_expand_kernel.md section 5): one block of 32 warps — rounds of
-   1024 parents — takes 13 % less kernel time than two blocks of 16 with the same 32 resident warps: the end-of-round tail (the
-   barrier stall of section 4) halves, and all warps of the SM run the same phase, so they share the instruction cache lines of the
-   scan.  The pool item keeps 16 bits: thread (10) | candidate offset in its group (6), which bounds a group at 63 candidates. */
+   (2 x <= 113 KB).  One block of 32 warps — rounds of 1024 parents — rather than two blocks of 16 with the same 32 resident warps:
+   the end-of-round tail (the barrier stall) halves, and all warps of the SM run the same phase, so they share the instruction
+   cache lines of the scan.  The pool item keeps 16 bits: thread (10) | candidate offset in its group (6), which bounds a group at 63 candidates. */
 template <class L> struct ExpandCfg {
     static constexpr size_t SMEM_ONE = 227 * 1024 - 512, SMEM_TWO = 113 * 1024;
     static constexpr int max_grp() { int m = 0; for (int g = 0; g < Ops<L>::NGRP; g++) m = Ops<L>::grp_size(g) > m ? Ops<L>::grp_size(g) : m; return m; }
@@ -326,10 +328,9 @@ template <class L> struct ExpandCfg {
  *          a block pool grouped by action (packed warp prefix sums, one shared atomic per warp and group, one barrier).
  *   apply  after the second barrier, warps take batches of 32 pairs of ONE group and apply them one per lane: no
  *          divergence between actions inside a warp, full lanes except one partial batch per group.
- * History, all measured on the shipped VSR.cfg (profiles/round1_expand_kernel.md): (1) every warp walking guards and
- * effects on its own: 88 kB of SASS against the instruction cache, 55 % `no_instruction` stall samples; (2) guards in a
- * run-time loop over candidates with one ballot + barrier per group: 75 warp instructions per (32 states, candidate)
- * for slot decoding and shared-memory field reads; (3) this form: 16 per candidate, 46 % fewer instructions overall.
+ * Earlier forms: (1) every warp walking guards and effects on its own: 88 kB of SASS against the instruction cache;
+ * (2) guards in a run-time loop over candidates with one ballot + barrier per group: 75 warp instructions per
+ * (32 states, candidate) for slot decoding and shared-memory field reads; (3) this form: 16 per candidate.
  */
 /* MULTI: the instantiation for several GPUs (push_records in emit, drain after the rounds).  The one-GPU instantiation has none
    of that code: it costs the hot path registers (380 vs 140 bytes of spills in emit at the 64-register budget). */
@@ -394,8 +395,8 @@ template <class L, bool MULTI> struct Expander {
 
     /* fingerprint, route, insert, stage: the part of apply that does not depend on the action */
     /* this lane's scratch row for the successor it builds: staging rows 32..63 are free whenever a batch starts (fewer than
-       32 states are staged then).  Plain rows, bank conflicts avoided by skewing the row STARTS (measured against rotating
-       every access: 7.5 % less kernel time on the shipped VSR.cfg, profiles/round2_expand_kernel.md).  Rows of
+       32 states are staged then).  Plain rows, bank conflicts avoided by skewing the row STARTS (rather than rotating
+       every access).  Rows of
        NW words collide every p = 32 / gcd(NW, 32) lanes; shifting lane l's row by l / p words puts the 32 lanes' word i in
        32 different banks, and an access is base + i: no per-access arithmetic. */
     typedef uint32_t* Row;
@@ -569,10 +570,8 @@ template <class L, bool MULTI> struct Expander {
     /* ---- drain: one record received from a peer per lane (world > 1), after this block's share of the frontier.  The
        sender computed the fingerprint; check hash and aux key are recomputed from the words; then the same seen-set insert
        / invariant / staging as a local successor.  drain_begin issues the header and bucket loads, drain_end consumes them.
-       Measured (tools/drain_bench.py, profiles/round2_multi_gpu.md): push + drain cost 53 ps per record, i.e. the drain
-       runs close to the seen-set's random-access ceiling; what did NOT help: 2 or 4 records in flight per lane (+15 % /
-       +60 %: register spills), and pipelining a chunk under every batch of the expansion (+19 %, and +5 % on ONE GPU,
-       again through spills in the hot loop). */
+       One record in flight per lane: more (2 or 4), or pipelining a chunk under every batch of the expansion, costs
+       register spills in the hot loop (tools/drain_bench.py measures the drain). */
     struct DrainPre {
         uint64_t fp, tm;
         unsigned long long home;

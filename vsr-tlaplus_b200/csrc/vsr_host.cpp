@@ -114,7 +114,7 @@ static bool load_layout_plugin(int R, int V, int K, LayoutPlugin* out, std::stri
         const char* nv = getenv("VSR_B200_NVCC");
         std::string nvcc = nv ? nv : (access("/usr/local/cuda/bin/nvcc", X_OK) == 0 ? "/usr/local/cuda/bin/nvcc" : "nvcc");
         const std::string tmp = path + ".tmp" + std::to_string((long)getpid()), log = path + ".log";
-        const std::string cmd = nvcc + " -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -diag-suppress 128"
+        const std::string cmd = nvcc + " -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -diag-suppress 128"
                                 " -DVSR_ONLY_R=" + std::to_string(R) + " -DVSR_ONLY_V=" + std::to_string(V) + " -DVSR_ONLY_K=" + std::to_string(K) +
                                 " -shared -Xlinker -Bsymbolic -o '" + tmp + "' '" + src + "' > '" + log + "' 2>&1";
         const int rc = system(cmd.c_str());

@@ -4,7 +4,7 @@
  * libvsr_b200.so carries the layouts of VSR_FOR_EACH_CONFIG (vsr_model.h).  The reference tells its user to edit the
  * constants of VSR.cfg (README.md:11-18 of the reference); for constants outside that list the loader (vsr_host.cpp,
  * load_layout_plugin) compiles this file once with
- *     nvcc -gencode arch=compute_100a,code=sm_100a -DVSR_ONLY_R=<ReplicaCount> -DVSR_ONLY_V=<|Values|>
+ *     nvcc -gencode arch=compute_90a,code=sm_90a -DVSR_ONLY_R=<ReplicaCount> -DVSR_ONLY_V=<|Values|>
  *          -DVSR_ONLY_K=<1 + StartViewOnTimerLimit> -shared -o layouts/libvsr_layout_R_V_K.so vsr_layout_plugin.cu
  * and takes the two vtables from it.  Same templates as the built-in layouts: nothing here but the instantiation.
  */
