@@ -24,8 +24,6 @@ build() { # name, flags
 build base ""                            # the default: one block of up to 32 warps per SM, pool fast path
 build warps16 "-DVSR_FORCE_WARPS=16"     # two blocks of 16 warps per SM (the shape until the re-entry session's A/B: +13 % kernel time)
 build invskip "-DVSR_EXP_INVSKIP"        # inline invariant only after the action groups that can falsify it (they rewrite a log / acknowledge a value)
-build casfirst "-DVSR_EXP_CASFIRST"       # no probe load: the first access of the home bucket is the CAS of its first slot
-build casinv "-DVSR_EXP_CASFIRST -DVSR_EXP_INVSKIP"
 build nopushfast "-DVSR_EXP_NO_PUSHFAST" # pool layout with the per-pair bound test always (+0.8 %)
 if [ -n "$VSR_VARIANTS_ALL" ]; then
 build bucket1 "-DVSR_BUCKET=1"           # seen-set probe = one 128-bit load of one entry (round 1); default is the 2-entry sector bucket

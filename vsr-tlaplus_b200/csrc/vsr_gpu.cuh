@@ -166,13 +166,14 @@ __device__ __forceinline__ uint64_t make_meta(int level, uint32_t auxkey, uint32
 }
 
 /* lock-free insert-if-absent over 16-byte entries {fp, meta}.  A probe reads one BUCKET of VSR_BUCKET consecutive entries
-   (1: one 128-bit load; 2: a whole 32-byte sector, read by ld256_cg as two 128-bit loads issued back to back — sm_90 has no
-   256-bit load; 4: two such sectors, all four loads issued together) and walks to
-   the next bucket only when every slot of this one holds another state: the kernel is bound by the LATENCY of dependent
-   probes, so a wider first probe is paid for in bandwidth the kernel does not use.
-   Slots of a bucket fill in order (no deletions), so a lookup may stop at the first empty slot.  The bucket's entries
-   are loaded by the caller as early as the fingerprint is known so that the HBM round trip overlaps the rest of the
-   successor's work. */
+   (1: one 128-bit load; 2: one 32-byte sector; 4: two sectors, read by ld256_cg, all four 128-bit loads issued together) and
+   walks to the next bucket only when every slot of this one holds another state.
+   Slots of a bucket fill in order (no deletions), so a lookup may stop at the first empty slot.  The bucket's first entry
+   (for VSR_BUCKET 4: all of it) is loaded by the caller as early as the fingerprint is known so that the HBM round trip
+   overlaps the rest of the successor's work.  With 2-entry buckets the second entry is read only when the first holds
+   another state: it is in L2 by then (same sector), and most inserts and duplicates end at the first entry.  Every
+   128-bit load of a warp gathers 32 random sectors, and those gathers bind the kernel: reading the whole sector up front
+   cost 9 % of the kernel time on an H100 (profiles/probe_gathers_h100.md). */
 #ifndef VSR_BUCKET
 #define VSR_BUCKET 2
 #endif
@@ -192,7 +193,7 @@ __device__ __forceinline__ void probe_load(const uint64_t* table, unsigned long 
 #if VSR_BUCKET == 1
     ld128_cg(table + 2 * h, p.e[0], p.e[1]);
 #elif VSR_BUCKET == 2
-    ld256_cg(table + 2 * h, p.e[0], p.e[1], p.e[2], p.e[3]);
+    ld128_cg(table + 2 * h, p.e[0], p.e[1]); /* the bucket's first entry only: table_insert_from reads the second on demand */
 #elif VSR_BUCKET == 4
     ld256_cg(table + 2 * h, p.e[0], p.e[1], p.e[2], p.e[3]);
     ld256_cg(table + 2 * h + 4, p.e[4], p.e[5], p.e[6], p.e[7]);
@@ -207,7 +208,13 @@ __device__ __forceinline__ int table_insert_from(uint64_t* table, unsigned long 
         probes++;
 VSR_UNROLL
         for (int j = 0; j < VSR_BUCKET; j++) {
-            uint64_t e0 = p.e[2 * j], e1 = p.e[2 * j + 1];
+            uint64_t e0, e1;
+            if (VSR_BUCKET == 2 && j == 1) {
+                ld128_cg(table + 2 * (h + 1), e0, e1); /* the first entry holds another state */
+            } else {
+                e0 = p.e[2 * j];
+                e1 = p.e[2 * j + 1];
+            }
             if (e0 == 0) {
                 cas128(table + 2 * (h + j), fp, meta, e0, e1);
                 if (e0 == 0 && e1 == 0) return INS_NEW;
@@ -227,26 +234,6 @@ VSR_UNROLL
         probe_load(table, h, p);
     }
 }
-#if defined(VSR_EXP_CASFIRST) && VSR_BUCKET == 2
-/* experiment (tools/variants.sh casfirst): no probe load — the first access of the home bucket IS the compare-and-swap of its
-   first slot.  A new state whose home slot is free is in after ONE round trip instead of two (load, then CAS), a duplicate
-   sitting in the home slot is recognised from the CAS's return value; only a home slot held by another state costs the second
-   access (the bucket's other slot).  Every access becomes an atomic. */
-__device__ __forceinline__ int table_insert_casfirst(uint64_t* table, unsigned long long cap, unsigned long long h, uint64_t fp, uint64_t meta,
-                                                     unsigned& probes, unsigned& collisions) {
-    Probe p;
-    cas128(table + 2 * h, fp, meta, p.e[0], p.e[1]);
-    if (p.e[0] == 0 && p.e[1] == 0) { probes++; return INS_NEW; }
-    if (p.e[0] == fp && (uint32_t)p.e[1] == (uint32_t)meta) {
-        probes++;
-        const bool same_level = (p.e[1] >> 56) == (meta >> 56);
-        const bool same_aux = ((p.e[1] >> 32) & 0xFFFFFF) == ((meta >> 32) & 0xFFFFFF);
-        return (same_level && !same_aux) ? INS_TIE : INS_DUP;
-    }
-    ld128_cg(table + 2 * (h + 1), p.e[2], p.e[3]);
-    return table_insert_from(table, cap, h, p, fp, meta, probes, collisions);
-}
-#endif
 __device__ __forceinline__ int table_insert(uint64_t* table, unsigned long long cap, uint64_t fp, uint64_t meta,
                                             unsigned& probes, unsigned& collisions) {
     const unsigned long long h = table_home(cap, fp);
@@ -474,12 +461,7 @@ template <class L, bool MULTI> struct Expander {
         if (live) {
             const uint64_t meta = make_meta(P.level, auxkey, chk);
             gen = mult;
-#if defined(VSR_EXP_CASFIRST) && VSR_BUCKET == 2
-            (void)first;
-            const int r = table_insert_casfirst(P.table, P.table_cap, home, fp, meta, probes, coll);
-#else
             const int r = table_insert_from(P.table, P.table_cap, home, first, fp, meta, probes, coll);
-#endif
             isnew = r == INS_NEW;
             if (r == INS_FULL) atomicExch(&P.ctr->overflow, 4);
             if (isnew && check_inv) bad = O_::invariant(P.run, v);
@@ -550,9 +532,7 @@ template <class L, bool MULTI> struct Expander {
                     /* start the seen-set probe now; the check hash, aux key and tags are computed under its latency */
                     live = true;
                     home = table_home(P.table_cap, fp);
-#if !(defined(VSR_EXP_CASFIRST) && VSR_BUCKET == 2)
                     probe_load(P.table, home, first);
-#endif
                     chk = check_hash<L>(v, P.run.use_view != 0);
                     auxkey = O_::aux_key(v);
                 } else {
@@ -603,9 +583,7 @@ template <class L, bool MULTI> struct Expander {
             d.fp = ((uint64_t)h.y << 32) | h.x;
             d.tm = ((uint64_t)h.w << 32) | h.z;
             d.home = table_home(P.table_cap, d.fp);
-#if !(defined(VSR_EXP_CASFIRST) && VSR_BUCKET == 2)
             probe_load(P.table, d.home, d.first);
-#endif
         }
         return d;
     }
