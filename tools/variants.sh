@@ -25,6 +25,8 @@ build base ""                            # the default: one block of up to 32 wa
 build warps16 "-DVSR_FORCE_WARPS=16"     # two blocks of 16 warps per SM (the shape until the re-entry session's A/B: +13 % kernel time)
 build invskip "-DVSR_EXP_INVSKIP"        # inline invariant only after the action groups that can falsify it (they rewrite a log / acknowledge a value)
 build nopushfast "-DVSR_EXP_NO_PUSHFAST" # pool layout with the per-pair bound test always (+0.8 %)
+build roundclk "-DVSR_EXP_ROUNDCLK"      # per-level split of the expand warps' cycles (end-of-round barrier, scan barriers, batches, scan) on stderr
+build passes1 "-DVSR_ROUND_PASSES=1"     # one scan pass per round (the shape before profiles/round_tail_h100.md)
 if [ -n "$VSR_VARIANTS_ALL" ]; then
 build bucket1 "-DVSR_BUCKET=1"           # seen-set probe = one 128-bit load of one entry (round 1); default is the 2-entry sector bucket
 build bucket4 "-DVSR_BUCKET=4"           # 4-entry bucket, two 256-bit loads issued together

@@ -373,6 +373,15 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
     li.overflow = c.overflow;
     li.ms = e->level_ms_acc;
     li.ms_insert = e->level_ms_insert_acc;
+#ifdef VSR_EXP_ROUNDCLK
+    { /* the last expand launch's warp-cycles by phase (one launch per level on one GPU) */
+        double all = 0;
+        for (int i = 0; i < 5; i++) all += (double)c.roundclk[i];
+        if (all > 0)
+            fprintf(stderr, "roundclk rank %d depth %d  ms %.4f  warp-Gcycles %.4f  end_barrier %.4f  scan_barriers %.4f  batches %.4f  scan %.4f  other %.4f\n",
+                    e->rank, e->level, e->level_ms_acc, all * 1e-9, c.roundclk[0] / all, c.roundclk[1] / all, c.roundclk[2] / all, c.roundclk[3] / all, c.roundclk[4] / all);
+    }
+#endif
     if (c.overflow) {
         snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (%s): %llu new states this level, frontier capacity %llu",
                  c.overflow == 1 ? "frontier" : (c.overflow == 2 ? "tie list" : (c.overflow == 3 ? "send buffer" : "seen-set")), (unsigned long long)c.out_count,

@@ -49,7 +49,15 @@ struct DevCounters {
     unsigned long long work_next;   /* next round of frontier states to hand out */
     unsigned long long drain_next;  /* next chunk of inbox records to hand out */
     unsigned int send_count[8];     /* records pushed to each rank by this launch (MAX_WORLD) */
+#ifdef VSR_EXP_ROUNDCLK
+    unsigned long long roundclk[5]; /* warp-cycles of this launch by phase (CLK_*); printed per level by the host */
+#endif
 };
+#ifdef VSR_EXP_ROUNDCLK
+/* phases of an expand warp's time: waiting at the end-of-round barrier, waiting at the scan's barriers (parents loaded,
+   qcount final, pool written), applying batches, scanning (parent load, guards, pool layout), and the rest (start, drain, final flush) */
+enum { CLK_END = 0, CLK_SCANBAR = 1, CLK_BATCH = 2, CLK_SCAN = 3, CLK_OTHER = 4 };
+#endif
 
 /* a same-level VIEW tie (SURVEY H2): header, then the candidate's L::NW packed words */
 struct TieRec {
@@ -258,46 +266,56 @@ template <int NW> __device__ __forceinline__ uint32_t* out_state(const ExpandPar
 
 /* ------------------------------------------------------------------ expand kernel */
 
-constexpr int SCAP = 64;      /* staged new states per warp */
 #ifdef VSR_QPS
 constexpr int QPS = VSR_QPS;  /* tools/variants.sh "qps1": a pool so small that the overflow path (leftovers) runs all the time */
 #else
 constexpr int QPS = 10;       /* pool entries per parent state (pool = QPS * states per block round) */
 #endif
 
-template <class L> struct WarpStage {
-    alignas(16) uint32_t stage[SCAP * L::NW + 32]; /* new states, packed back to back for the bulk store (+ room for the skew of the scratch rows, Expander::scratch) */
-    unsigned long long tstage[SCAP];             /* their trace records */
+/* a warp's staging area of ROWS rows: new states, packed back to back for the bulk store; its last 32 rows are the lanes'
+   scratch rows while a batch builds its successors.  ROWS 64: flushed 32 states at a time (Expander::commit).  ROWS 32:
+   every batch flushes all its new states, which halves the area; the two-pass round needs that space */
+template <class L, int ROWS> struct WarpStage {
+    alignas(16) uint32_t stage[ROWS * L::NW + 32]; /* (+ room for the skew of the scratch rows, Expander::scratch) */
+    unsigned long long tstage[ROWS];             /* their trace records */
     /* per-warp running state.  It lives here, not in the Expander object: the big per-action routines are real calls
        (one copy of each in the instruction cache), and an object whose address is passed to them would be kept in
        local memory — 1024 threads x a few hundred bytes does not fit the L1 left beside 220 KB of shared memory. */
     int sn;                                      /* states currently staged */
 };
-template <class L, int WARPS> struct BlockSmemT {
-    static constexpr int NS = WARPS * 32;        /* parent states per block round: one per thread */
+template <class L, int WARPS, int PASSES> struct BlockSmemT {
+    typedef WarpStage<L, PASSES == 2 ? 32 : 64> Stage;
+    static constexpr int NS = WARPS * 32;        /* parent states per scan pass: one per thread */
+    static constexpr int NR = PASSES * NS;       /* parent states per block round */
     static constexpr int NG = 13;                /* action groups (Ops<L>::NGRP) */
     uint64_t fp_tab[8 * 256];                    /* FP64 slicing-by-8 tables */
-    uint32_t par[NS * (L::NW + 1)];              /* parents, row stride NW+1 (odd: bank-conflict-free column reads) */
-    static constexpr int QCAP = QPS * NS;
-    uint16_t pool[QCAP];                         /* enabled (state, candidate) pairs, grouped by action */
-    int qcount[NG];                              /* pairs found per group (may exceed what the pool holds) */
+    uint32_t par[NR * (L::NW + 1)];              /* parents, row stride NW+1 (odd: bank-conflict-free column reads) */
+    static constexpr int QCAP = QPS * NS;        /* pool entries per pass */
+    uint16_t pool[PASSES * QCAP];                /* enabled (state, candidate) pairs, by pass, then grouped by action */
+    int qcount[PASSES][NG];                      /* pairs found per pass and group (may exceed what the pool holds) */
     int take;
     unsigned long long round_first;
-    WarpStage<L> w[WARPS];
+    Stage w[WARPS];
 };
 /* Block shape.  ONE block of up to 32 warps per SM when its shared memory fits (227 KB), else two blocks of 16 / 12 / 8 warps
    (2 x <= 113 KB).  One block of 32 warps — rounds of 1024 parents — rather than two blocks of 16 with the same 32 resident warps:
    the end-of-round tail (the barrier stall) halves, and all warps of the SM run the same phase, so they share the instruction
-   cache lines of the scan.  The pool item keeps 16 bits: thread (10) | candidate offset in its group (6), which bounds a group at 63 candidates. */
+   cache lines of the scan.  The pool item keeps 16 bits: thread (10) | candidate offset in its group (6), which bounds a group at 63 candidates.
+   Two scan passes per round when the shared memory holds them (one block per SM only): rounds of 2 x 32 x WARPS parents, so
+   the end-of-round barrier, where every warp waits for the slowest warp's last batch, comes once per two passes.  It took
+   12 % of the warp-cycles at one pass per round on an H100 (profiles/round_tail_h100.md).  The two-pass round uses the
+   32-row staging area (a flush per batch) to fit; the warps are counted with the one-pass block, so both shapes have the
+   same warps and register budget.  A flush per batch costs where a batch finds few new states: 6-9 % on five replicas
+   (g ~ 7), so one-pass layouts keep the 64-row area. */
 template <class L> struct ExpandCfg {
     static constexpr size_t SMEM_ONE = 227 * 1024 - 512, SMEM_TWO = 113 * 1024;
     static constexpr int max_grp() { int m = 0; for (int g = 0; g < Ops<L>::NGRP; g++) m = Ops<L>::grp_size(g) > m ? Ops<L>::grp_size(g) : m; return m; }
     template <int W> static constexpr int pick_one() { /* most warps (even) of ONE block per SM; 0: not even 18 fit */
         if constexpr (W < 18) return 0;
-        else if constexpr (sizeof(BlockSmemT<L, W>) <= SMEM_ONE) return W;
+        else if constexpr (sizeof(BlockSmemT<L, W, 1>) <= SMEM_ONE) return W;
         else return pick_one<W - 2>();
     }
-    static constexpr int W2 = sizeof(BlockSmemT<L, 16>) <= SMEM_TWO ? 16 : (sizeof(BlockSmemT<L, 12>) <= SMEM_TWO ? 12 : 8);
+    static constexpr int W2 = sizeof(BlockSmemT<L, 16, 1>) <= SMEM_TWO ? 16 : (sizeof(BlockSmemT<L, 12, 1>) <= SMEM_TWO ? 12 : 8);
     static constexpr int W1 = max_grp() < 64 ? pick_one<32>() : 0;
 #ifdef VSR_FORCE_WARPS
     static constexpr int WARPS = VSR_FORCE_WARPS; /* tuning experiments only */
@@ -305,7 +323,12 @@ template <class L> struct ExpandCfg {
     static constexpr int WARPS = W1 >= 2 * W2 - 4 ? W1 : W2; /* one block unless it would cost more than 4 resident warps */
 #endif
     static constexpr int BLOCKS = WARPS > 16 ? 1 : 2;
-    typedef BlockSmemT<L, WARPS> Smem;
+#ifdef VSR_ROUND_PASSES
+    static constexpr int PASSES = VSR_ROUND_PASSES; /* A/B: tools/variants.sh "passes1" */
+#else
+    static constexpr int PASSES = BLOCKS == 1 && sizeof(BlockSmemT<L, WARPS, 2>) <= SMEM_ONE ? 2 : 1;
+#endif
+    typedef BlockSmemT<L, WARPS, PASSES> Smem;
 };
 
 /*
@@ -324,20 +347,42 @@ template <class L> struct ExpandCfg {
 template <class L, bool MULTI> struct Expander {
     typedef Ops<L> O_;
     typedef typename ExpandCfg<L>::Smem Smem;
-    static constexpr int WARPS = ExpandCfg<L>::WARPS, NS = Smem::NS;
+    typedef typename Smem::Stage Stage;
+    static constexpr int WARPS = ExpandCfg<L>::WARPS, NS = Smem::NS, PASSES = ExpandCfg<L>::PASSES;
+    static constexpr int SROWS = PASSES == 2 ? 32 : 64; /* the staging area's rows (WarpStage) */
     const ExpandParams& P;
     Smem& B;
-    WarpStage<L>& S;
+    Stage& S;
     const int lane, warp, tid;
     const uint32_t* mine = nullptr;
     bool have = false;
+    int pass = 0; /* the round's scan pass in progress: this thread scans parent pass * NS + tid */
+    __device__ __forceinline__ int pass_i() const { return PASSES == 1 ? 0 : pass; } /* a constant for one-pass layouts */
 
-    __device__ Expander(const ExpandParams& p, Smem& b) : P(p), B(b), S(b.w[threadIdx.x >> 5]), lane(threadIdx.x & 31), warp(threadIdx.x >> 5), tid(threadIdx.x) {}
+    __device__ Expander(const ExpandParams& p, Smem& b) : P(p), B(b), S(b.w[threadIdx.x >> 5]), lane(threadIdx.x & 31), warp(threadIdx.x >> 5), tid(threadIdx.x) {
+#ifdef VSR_EXP_ROUNDCLK
+        clk_t = clock64();
+#endif
+    }
+
+#ifdef VSR_EXP_ROUNDCLK
+    /* tools/variants.sh "roundclk": where each warp's cycles go.  clk_mark(i) books the cycles since the previous mark
+       to phase i (CLK_*); finish() adds the warp's sums to DevCounters::roundclk */
+    unsigned long long clk_t = 0, clk[5] = {};
+    __device__ __forceinline__ void clk_mark(int i) {
+        const unsigned long long t = clock64();
+        clk[i] += t - clk_t;
+        clk_t = t;
+    }
+#define VSR_CLK(X, i) (X).clk_mark(CLK_##i)
+#else
+#define VSR_CLK(X, i) ((void)0)
+#endif
 
     /* flush the first n staged states (n <= 32) to the next frontier: one atomicAdd for the block of
        ids, one TMA bulk store for the states, then move the remainder (< 32 states) down */
-    static __device__ __noinline__ void flush(const ExpandParams& P, WarpStage<L>& S, int lane, int n) {
-        const int sn = S.sn;
+    static __device__ __noinline__ void flush(const ExpandParams& P, Stage& S, int lane, int n) {
+        const int sn = SROWS == 32 ? n : S.sn; /* 32 rows: the whole batch, nothing to move down */
         unsigned long long base = 0;
         if (lane == 0) base = atomicAdd(&P.ctr->out_count, (unsigned long long)n);
         base = __shfl_sync(0xffffffffu, base, 0);
@@ -381,24 +426,24 @@ template <class L, bool MULTI> struct Expander {
     }
 
     /* fingerprint, route, insert, stage: the part of apply that does not depend on the action */
-    /* this lane's scratch row for the successor it builds: staging rows 32..63 are free whenever a batch starts (fewer than
-       32 states are staged then).  Plain rows, bank conflicts avoided by skewing the row STARTS (rather than rotating
-       every access).  Rows of
+    /* this lane's scratch row for the successor it builds: the last 32 staging rows are free whenever a batch starts (a
+       64-row area holds fewer than 32 staged states then, a 32-row area none).  Plain rows, bank conflicts avoided by skewing the row STARTS (rather than
+       rotating every access).  Rows of
        NW words collide every p = 32 / gcd(NW, 32) lanes; shifting lane l's row by l / p words puts the 32 lanes' word i in
        32 different banks, and an access is base + i: no per-access arithmetic. */
     typedef uint32_t* Row;
     static constexpr int gcd32(int a) { int g = 32; while (a % g) g >>= 1; return g; }
     static constexpr int SKEW_P = 32 / gcd32(L::NW);
-    static __device__ __forceinline__ Row scratch(WarpStage<L>& S, int lane) { return &S.stage[(32 + lane) * L::NW + lane / SKEW_P]; }
+    static __device__ __forceinline__ Row scratch(Stage& S, int lane) { return &S.stage[(SROWS - 32 + lane) * L::NW + lane / SKEW_P]; }
 
     /* Records for peer ranks (world > 1), pushed by the kernel itself: the lanes of the batch whose successor belongs to
-       another rank lay their records out in destination order in the free half of the warp's staging area (every lane
-       has read its scratch row into registers by now), each destination's run takes its slots in that rank's inbox with
-       ONE atomicAdd on a local counter, and the run leaves as ONE TMA bulk store (cp.async.bulk.global.shared::cta) to
-       the peer's memory — over NVLink when push[] is a peer mapping.  Fire and forget: nothing waits for the remote
-       write, the owner inserts the records in its next launch (drain).  The scratch half holds CAPREC records; a batch
-       with more senders goes in two passes. */
-    static __device__ __forceinline__ void push_records(const ExpandParams& P, WarpStage<L>& S, int lane, const RegRow<L::NW>& v, int send_to, uint64_t fp,
+       another rank lay their records out in destination order in the warp's 32 scratch rows (every lane has read its
+       scratch row into registers by now, and the batch's new states are staged only after this), each destination's run
+       takes its slots in that rank's inbox with ONE atomicAdd on a local counter, and the run leaves as ONE TMA bulk store
+       (cp.async.bulk.global.shared::cta) to the peer's memory — over NVLink when push[] is a peer mapping.  Fire and
+       forget: nothing waits for the remote write, the owner inserts the records in its next launch (drain).  The rows hold
+       CAPREC records; a batch with more senders goes in two passes. */
+    static __device__ __forceinline__ void push_records(const ExpandParams& P, Stage& S, int lane, const RegRow<L::NW>& v, int send_to, uint64_t fp,
                                                         uint64_t tm) {
         const unsigned senders = __ballot_sync(0xffffffffu, send_to >= 0);
         if (!senders) return;
@@ -427,7 +472,7 @@ template <class L, bool MULTI> struct Expander {
             return;
         }
         const int pos = off + rnk, total = __popc(senders);
-        uint32_t* sbuf = &S.stage[32 * L::NW];
+        uint32_t* sbuf = &S.stage[(SROWS - 32) * L::NW];
         for (int lo = 0; lo < total; lo += CAPREC) {
             const int hi = lo + CAPREC < total ? lo + CAPREC : total;
             if (send_to >= 0 && pos >= lo && pos < hi) {
@@ -451,11 +496,11 @@ template <class L, bool MULTI> struct Expander {
        survivors into the warp's staging area, flush — shared by the expansion (emit) and by the records received from
        peers (drain).  Returns this lane's counts for the run's statistics: successors generated (low half) | seen-set
        probes (high half); the caller keeps the running sums in registers (a warp reduction per batch cost 25 shuffles) */
-    static __device__ __forceinline__ unsigned long long commit(const ExpandParams& P, WarpStage<L>& S, int lane, const RegRow<L::NW>& v, bool live, uint64_t fp,
+    static __device__ __forceinline__ unsigned long long commit(const ExpandParams& P, Stage& S, int lane, const RegRow<L::NW>& v, bool live, uint64_t fp,
                                                                 uint32_t chk, uint32_t auxkey, unsigned long long home, const Probe& first, unsigned long long trec,
                                                                 unsigned mult, bool check_inv = true) {
         unsigned gen = 0, probes = 0, coll = 0;
-        int sn = S.sn;
+        int sn = SROWS == 32 ? 0 : S.sn;
         bool isnew = false;
         int bad = 0;
         if (live) {
@@ -495,17 +540,21 @@ template <class L, bool MULTI> struct Expander {
         }
         sn += __popc(newmask);
         __syncwarp();
-        if (lane == 0) S.sn = sn;
-        __syncwarp();
-        while (sn >= 32) {
-            flush(P, S, lane, 32);
-            sn -= 32;
+        if constexpr (SROWS == 32) { /* flush the whole batch: nothing stays staged (S.sn stays 0) */
+            if (newmask) flush(P, S, lane, sn);
+        } else {
+            if (lane == 0) S.sn = sn;
+            __syncwarp();
+            while (sn >= 32) {
+                flush(P, S, lane, 32);
+                sn -= 32;
+            }
         }
         return (unsigned long long)gen | ((unsigned long long)probes << 32);
     }
 
     /* fingerprint and route one successor per lane: the part of apply that does not depend on the action */
-    static __device__ __noinline__ unsigned long long emit(const ExpandParams& P, Smem& B, WarpStage<L>& S, int lane, const Row n, int mult,
+    static __device__ __noinline__ unsigned long long emit(const ExpandParams& P, Smem& B, Stage& S, int lane, const Row n, int mult,
                                                            int cand, int si, bool act, bool check_inv) {
         int send_to = -1;
         uint64_t fp = 0;
@@ -645,14 +694,15 @@ template <class L, bool MULTI> struct Expander {
             while (mm) {
                 const int bit = __ffs(mm) - 1;
                 mm &= mm - 1;
-                if (FAST || pos < Smem::QCAP) B.pool[pos] = (uint16_t)(tid | ((k * 32 + bit) << TBITS));
+                if (FAST || pos < Smem::QCAP) B.pool[pass_i() * Smem::QCAP + pos] = (uint16_t)(tid | ((k * 32 + bit) << TBITS));
                 else left |= 1u << bit;
                 pos++;
             }
             if (!FAST) m[moff(G) + k] = left;
         }
         if constexpr (G + 1 < NG) {
-            const int nst = FAST ? st + B.qcount[G] : (st + B.qcount[G] < Smem::QCAP ? st + B.qcount[G] : Smem::QCAP);
+            const int q = B.qcount[pass_i()][G];
+            const int nst = FAST ? st + q : (st + q < Smem::QCAP ? st + q : Smem::QCAP);
             push<G + 1, FAST>(m, ex, wb, nst);
         }
     }
@@ -668,7 +718,7 @@ template <class L, bool MULTI> struct Expander {
                     m[moff(G) + k] &= m[moff(G) + k] - 1;
                     cand = O_::grp_begin(G) + k * 32 + bit;
                 }
-                tally(apply<G>(P, B, S, lane, mine, cand, tid, inl));
+                tally(apply<G>(P, B, S, lane, mine, cand, pass_i() * NS + tid, inl));
             }
         }
         if constexpr (G + 1 < NG) leftovers<G + 1>(m);
@@ -707,17 +757,19 @@ template <class L, bool MULTI> struct Expander {
         VSR_UNROLL
         for (int i = 0; i < PW; i++) { anyc |= pc[i]; ex[i] -= pc[i]; } /* inclusive -> exclusive */
         uint32_t mybase = 0;
-        if (lane < NG && mytot) mybase = (uint32_t)atomicAdd(&B.qcount[lane], (int)mytot);
+        if (lane < NG && mytot) mybase = (uint32_t)atomicAdd(&B.qcount[pass_i()][lane], (int)mytot);
         VSR_UNROLL
         for (int i = 0; i < PW; i++) wb[i] = 0;
         VSR_UNROLL
         for (int g = 0; g < NG; g++) wb[g >> 1] |= (__shfl_sync(0xffffffffu, mybase, g) & 0xFFFFu) << (16 * (g & 1));
-        if (P.check_deadlock && have && !anyc) atomicMin(&P.ctr->dead_id, P.in_base + B.round_first + tid);
+        if (P.check_deadlock && have && !anyc) atomicMin(&P.ctr->dead_id, P.in_base + B.round_first + pass_i() * NS + tid);
+        VSR_CLK(*this, SCAN);
         __syncthreads(); /* qcount[] final: group g's segment starts at min(sum of the groups before it, QCAP) */
+        VSR_CLK(*this, SCANBAR);
 #ifndef VSR_EXP_NO_PUSHFAST
         int all = 0;
         VSR_UNROLL
-        for (int g = 0; g < NG; g++) all += B.qcount[g];
+        for (int g = 0; g < NG; g++) all += B.qcount[pass_i()][g];
         if (all <= Smem::QCAP) { /* block-uniform: the usual case */
             push<0, true>(m, ex, wb, 0);
             return;
@@ -730,7 +782,7 @@ template <class L, bool MULTI> struct Expander {
         if (__any_sync(0xffffffffu, rest != 0)) leftovers<0>(m);
     }
     /* apply one (parent, candidate) pair of group G per lane; the only copy of that action's effect in the kernel */
-    template <int G> static __device__ __noinline__ unsigned long long apply(const ExpandParams& P, Smem& B, WarpStage<L>& S, int lane,
+    template <int G> static __device__ __noinline__ unsigned long long apply(const ExpandParams& P, Smem& B, Stage& S, int lane,
                                                                              const uint32_t* parent, int cand, int si, bool act) {
         const Row n = scratch(S, lane);
         int mult = 0;
@@ -743,14 +795,14 @@ template <class L, bool MULTI> struct Expander {
         return emit(P, B, S, lane, n, mult, cand, si, act, true);
 #endif
     }
-    /* one batch of <= 32 queued pairs of group G, pool[b .. b + k) */
-    template <int G> static __device__ __forceinline__ unsigned long long batch(const ExpandParams& P, Smem& B, WarpStage<L>& S, int lane, int b,
+    /* one batch of <= 32 queued pairs of group G, pool[b .. b + k) (all of one pass) */
+    template <int G> static __device__ __forceinline__ unsigned long long batch(const ExpandParams& P, Smem& B, Stage& S, int lane, int b,
                                                                                 int k) {
         const bool act = lane < k;
         int cand = 0, si = 0;
         if (act) {
             const unsigned item = B.pool[b + lane];
-            si = item & ((1 << TBITS) - 1);
+            si = (PASSES == 1 ? 0 : b / Smem::QCAP) * NS + (int)(item & ((1 << TBITS) - 1));
             cand = O_::grp_begin(G) + (int)(item >> TBITS);
         }
         return apply<G>(P, B, S, lane, &B.par[si * (L::NW + 1)], cand, si, act);
@@ -773,23 +825,35 @@ template <class L, bool MULTI> struct Expander {
                 B.par[(i / L::NW) * (L::NW + 1) + (i % L::NW)] = __ldg(row + i % L::NW);
             }
         }
-        if (tid < Smem::NG) B.qcount[tid] = 0;
+        if (tid < PASSES * Smem::NG) (&B.qcount[0][0])[tid] = 0;
         if (tid == 0) { B.round_first = first; B.take = 0; }
+        VSR_CLK(*this, SCAN);
         __syncthreads();
-        have = tid < count;
-        mine = &B.par[(have ? tid : 0) * (L::NW + 1)];
-        scan_all();
+        VSR_CLK(*this, SCANBAR);
+#pragma unroll 1
+        for (pass = 0; pass < PASSES; pass++) { /* a loop, not unrolled: one copy of the guards in the instruction cache */
+            have = pass_i() * NS + tid < count;
+            mine = &B.par[(have ? pass_i() * NS + tid : 0) * (L::NW + 1)];
+            scan_all();
+        }
+        VSR_CLK(*this, SCAN);
         __syncthreads();
-        /* batches: group g has ceil(|group g's pool segment| / 32) of them.  Lane g keeps group g's segment [st, en) and
-           the index of its first batch, so mapping a batch number to (group, offset) is one ballot and three shuffles. */
-        const int q = lane < Smem::NG ? B.qcount[lane] : 0;
+        VSR_CLK(*this, SCANBAR);
+        /* batches: segment s = (pass s / NG, group s % NG) has ceil(|its part of the pass's pool| / 32) of them.  Lane s keeps
+           segment s's pool range [st, en) and the index of its first batch, so mapping a batch number to (segment, offset) is
+           one ballot and three shuffles. */
+        static_assert(PASSES * Smem::NG <= 32, "one lane per segment");
+        const int sp = lane / Smem::NG; /* this lane's pass */
+        const int q = lane < PASSES * Smem::NG ? (&B.qcount[0][0])[lane] : 0;
         int inc = q;
         VSR_UNROLL
         for (int o = 1; o < 32; o <<= 1) {
             const int t = __shfl_up_sync(0xffffffffu, inc, o);
             if (lane >= o) inc += t;
         }
-        const int seg_st = inc - q < Smem::QCAP ? inc - q : Smem::QCAP, seg_en = inc < Smem::QCAP ? inc : Smem::QCAP;
+        const int before = __shfl_sync(0xffffffffu, inc, sp * Smem::NG - 1 + (sp == 0)); /* pairs of the passes before this lane's */
+        if (sp > 0) inc -= before;
+        const int seg_st = sp * Smem::QCAP + (inc - q < Smem::QCAP ? inc - q : Smem::QCAP), seg_en = sp * Smem::QCAP + (inc < Smem::QCAP ? inc : Smem::QCAP);
         const int nb = (seg_en - seg_st + 31) >> 5;
         int binc = nb;
         VSR_UNROLL
@@ -803,12 +867,12 @@ template <class L, bool MULTI> struct Expander {
             if (lane == 0) t = atomicAdd(&B.take, 1);
             t = __shfl_sync(0xffffffffu, t, 0);
             if (t >= total) break;
-            const int g = __popc(__ballot_sync(0xffffffffu, lane < Smem::NG && binc <= t)); /* groups that end before batch t */
-            const int st = __shfl_sync(0xffffffffu, seg_st, g), en = __shfl_sync(0xffffffffu, seg_en, g);
-            const int b = st + (t - __shfl_sync(0xffffffffu, binc - nb, g)) * 32;
+            const int s = __popc(__ballot_sync(0xffffffffu, lane < PASSES * Smem::NG && binc <= t)); /* segments that end before batch t */
+            const int st = __shfl_sync(0xffffffffu, seg_st, s), en = __shfl_sync(0xffffffffu, seg_en, s);
+            const int b = st + (t - __shfl_sync(0xffffffffu, binc - nb, s)) * 32;
             const int k = en - b < 32 ? en - b : 32;
             unsigned long long r;
-            switch (g) {
+            switch (s % Smem::NG) {
             case 0: r = batch<0>(P, B, S, lane, b, k); break;   case 1: r = batch<1>(P, B, S, lane, b, k); break;
             case 2: r = batch<2>(P, B, S, lane, b, k); break;   case 3: r = batch<3>(P, B, S, lane, b, k); break;
             case 4: r = batch<4>(P, B, S, lane, b, k); break;   case 5: r = batch<5>(P, B, S, lane, b, k); break;
@@ -818,11 +882,19 @@ template <class L, bool MULTI> struct Expander {
             default: r = batch<12>(P, B, S, lane, b, k); break;
             }
             tally(r);
+            VSR_CLK(*this, BATCH);
         }
+        VSR_CLK(*this, BATCH);
     }
 
     __device__ void finish() {
         while (S.sn > 0) flush(P, S, lane, S.sn < 32 ? S.sn : 32);
+#ifdef VSR_EXP_ROUNDCLK
+        clk_mark(CLK_OTHER);
+        VSR_UNROLL
+        for (int i = 0; i < 5; i++)
+            if (lane == 0) atomicAdd(&P.ctr->roundclk[i], clk[i]);
+#endif
         for (int o = 16; o; o >>= 1) {
             acc_gen += __shfl_xor_sync(0xffffffffu, acc_gen, o);
             acc_probes += __shfl_xor_sync(0xffffffffu, acc_probes, o);
@@ -841,30 +913,29 @@ template <class L, bool MULTI> __global__ void __launch_bounds__(ExpandCfg<L>::W
     for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) B.fp_tab[i] = P.fp_tab[i];
     __shared__ unsigned long long next_round;
     Expander<L, MULTI> X(P, B);
-    if ((threadIdx.x & 31) == 0) {
-        WarpStage<L>& S = B.w[threadIdx.x >> 5];
-        S.sn = 0;
-    }
-    const unsigned long long nrounds = (P.n_in + Smem::NS - 1) / Smem::NS;
+    if ((threadIdx.x & 31) == 0) B.w[threadIdx.x >> 5].sn = 0;
+    const unsigned long long nrounds = (P.n_in + Smem::NR - 1) / Smem::NR;
     if (threadIdx.x == 0) next_round = atomicAdd(&P.ctr->work_next, 1ull);
+    VSR_CLK(X, OTHER);
     for (;;) {
         __syncthreads();
         const unsigned long long c = next_round;
         __syncthreads();
+        VSR_CLK(X, END);
         if (c >= nrounds) break;
         /* claim the round after this one now: the global atomic's latency hides under this round's work */
         if (threadIdx.x == 0) {
             next_round = atomicAdd(&P.ctr->work_next, 1ull);
             /* pull the next round's parents into L2 while this round runs */
             const unsigned long long nx = next_round;
-            if (nx < nrounds && (nx + 1) * Smem::NS <= P.in_split) {
-                const unsigned long long nfirst = nx * Smem::NS;
-                const unsigned long long ncount = (P.n_in - nfirst) < (unsigned long long)Smem::NS ? (P.n_in - nfirst) : Smem::NS;
+            if (nx < nrounds && (nx + 1) * Smem::NR <= P.in_split) {
+                const unsigned long long nfirst = nx * Smem::NR;
+                const unsigned long long ncount = (P.n_in - nfirst) < (unsigned long long)Smem::NR ? (P.n_in - nfirst) : Smem::NR;
                 asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(P.in + nfirst * L::NW), "r"((uint32_t)(ncount * L::BYTES)) : "memory");
             }
         }
-        const unsigned long long first = c * Smem::NS;
-        const int count = (int)((P.n_in - first) < (unsigned long long)Smem::NS ? (P.n_in - first) : Smem::NS);
+        const unsigned long long first = c * Smem::NR;
+        const int count = (int)((P.n_in - first) < (unsigned long long)Smem::NR ? (P.n_in - first) : Smem::NR);
         X.run_round(first, count);
     }
     if (MULTI && P.drain_total) X.drain();
