@@ -217,6 +217,22 @@ int vsr_engine_reset(VsrEngine* e);
 const char* vsr_engine_last_error(const VsrEngine* e);
 /* with opts.collect_levels: number of states first seen at depth `level` (1-based) and, if host_out has room, a copy */
 uint64_t vsr_engine_collected(const VsrEngine* e, int level, void* host_out, uint64_t cap_states);
+/* Audit of the level just finished (tests): one device pass over this rank's seen-set and current frontier.
+ * tagged = seen-set entries whose level tag is `level`; found = frontier states whose (VIEW fingerprint, check hash) is in
+ * the seen-set with that tag; the digests are order-independent: sum and xor of mix64(VIEW fingerprint), and of a hash
+ * of all the state's words; tagged_fp_* are the same fingerprint digests over the tagged seen-set entries.  A correct level
+ * has found == tagged == size and equal fingerprint digests on both sides (a state written twice and another not at all
+ * keep the counts but not the digests). */
+typedef struct VsrLevelAudit {
+    uint64_t size, tagged, found;
+    uint64_t fp_sum, fp_xor, words_sum, words_xor;
+    uint64_t tagged_fp_sum, tagged_fp_xor;
+    int32_t level, _pad;
+} VsrLevelAudit;
+int vsr_engine_audit_level(VsrEngine* e, VsrLevelAudit* out);
+/* the expand kernel's shape for this model's layout (no GPU needed): warps per block, blocks per SM, scan passes per
+ * round, staging rows per warp */
+int vsr_expand_shape(const VsrModel* m, int* warps, int* blocks, int* passes, int* stage_rows);
 /* Rebuild the counterexample ending at local state id (single-rank engines). */
 int vsr_engine_build_trace(VsrEngine* e, uint64_t local_id, void* trace_out, uint8_t* trace_actions, size_t trace_cap);
 

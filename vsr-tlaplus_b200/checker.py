@@ -138,6 +138,14 @@ class VsrLevelInfo(C.Structure):
     ]
 
 
+class VsrLevelAudit(C.Structure):
+    _fields_ = [
+        ("size", C.c_uint64), ("tagged", C.c_uint64), ("found", C.c_uint64), ("fp_sum", C.c_uint64), ("fp_xor", C.c_uint64),
+        ("words_sum", C.c_uint64), ("words_xor", C.c_uint64), ("tagged_fp_sum", C.c_uint64), ("tagged_fp_xor", C.c_uint64),
+        ("level", C.c_int32), ("_pad", C.c_int32),
+    ]
+
+
 # every symbol include/vsr_b200.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = [
     "vsr_load", "vsr_load_cfg_text", "vsr_model_create", "vsr_model_free", "vsr_model_info", "vsr_init", "vsr_successors", "vsr_enabled_candidates",
@@ -146,7 +154,7 @@ EXPORTED_SYMBOLS = [
     "vsr_engine_record_bytes", "vsr_engine_seed_init", "vsr_engine_expand", "vsr_engine_expand_part", "vsr_engine_step",
     "vsr_engine_insert_records", "vsr_engine_finish_level", "vsr_engine_frontier_size", "vsr_engine_read_frontier",
     "vsr_engine_trace_record", "vsr_engine_stats", "vsr_engine_reset", "vsr_engine_checkpoint", "vsr_engine_recover", "vsr_engine_lookup", "vsr_engine_last_error", "vsr_engine_collected", "vsr_engine_build_trace",
-    "vsr_replay_candidates", "vsr_probe_bench", "vsr_simulate", "vsr_walk", "vsr_version",
+    "vsr_engine_audit_level", "vsr_expand_shape", "vsr_replay_candidates", "vsr_probe_bench", "vsr_simulate", "vsr_walk", "vsr_version",
     "vsr_group_open", "vsr_group_open_local", "vsr_group_close", "vsr_group_barrier", "vsr_group_allgather", "vsr_group_abort",
     "vsr_group_set_timeout", "vsr_group_rank", "vsr_group_world", "vsr_group_last_error",
     "vsr_engine_attach_group", "vsr_engine_attach_staged", "vsr_engine_detach", "vsr_engine_default_inbox_records",
@@ -234,6 +242,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.vsr_engine_collected.argtypes = [vp, C.c_int, vp, u64]
     lib.vsr_engine_collected.restype = u64
     lib.vsr_engine_build_trace.argtypes = [vp, u64, vp, C.POINTER(C.c_uint8), C.c_size_t]
+    lib.vsr_engine_audit_level.argtypes = [vp, C.POINTER(VsrLevelAudit)]
+    lib.vsr_expand_shape.argtypes = [vp] + [C.POINTER(C.c_int)] * 4
     lib.vsr_replay_candidates.argtypes = [vp, C.POINTER(C.c_uint32), C.c_int, vp, C.POINTER(C.c_uint8), C.c_size_t]
     lib.vsr_simulate.argtypes = [vp, C.POINTER(VsrSimOpts), C.POINTER(VsrSimStats), vp, C.POINTER(C.c_uint8), C.c_size_t]
     lib.vsr_walk.argtypes = [vp, u64, u64, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
@@ -361,6 +371,14 @@ class ModelChecker:
             self.close()
         except Exception:
             pass
+
+    def expand_shape(self) -> Tuple[int, int, int, int]:
+        """(warps per block, blocks per SM, scan passes per round, staging rows per warp) of this layout's expand kernel"""
+        v = [C.c_int() for _ in range(4)]
+        rc = self._lib.vsr_expand_shape(self._h, *[C.byref(x) for x in v])
+        if rc:
+            raise VsrError(rc, "no GPU kernels for this layout")
+        return tuple(int(x.value) for x in v)
 
     # -- single-state operations (host) -----------------------------------------------------------
     def _buf(self, n: int = 1):

@@ -470,6 +470,45 @@ int vsr_engine_lookup(VsrEngine* e, const void* state, int* level_out, int* owne
     return 0;
 }
 
+int vsr_engine_audit_level(VsrEngine* e, VsrLevelAudit* out) {
+    memset(out, 0, sizeof *out);
+    out->level = e->level;
+    out->size = e->n_cur;
+    AuditSums* d = nullptr;
+    CK(cudaMallocAsync((void**)&d, sizeof(AuditSums), e->stream));
+    ExpandParams p;
+    fill_params(e, p);
+    p.out = e->frontier[e->cur]; /* the level just finished, read as the expand kernel wrote it (host part included) */
+    p.out_hi = e->frontier_host[e->cur];
+    p.level = e->level;
+    cudaError_t ce = cudaMemsetAsync(d, 0, sizeof(AuditSums), e->stream);
+    if (ce == cudaSuccess) ce = e->g->launch_audit(p, e->n_cur, d, e->sms, e->stream);
+    AuditSums h;
+    memset(&h, 0, sizeof h);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(&h, d, sizeof h, cudaMemcpyDeviceToHost, e->stream);
+    cudaFreeAsync(d, e->stream);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->stream);
+    CK(ce);
+    out->tagged = h.tagged;
+    out->found = h.found;
+    out->fp_sum = h.fp_sum;
+    out->fp_xor = h.fp_xor;
+    out->words_sum = h.words_sum;
+    out->words_xor = h.words_xor;
+    out->tagged_fp_sum = h.tagged_fp_sum;
+    out->tagged_fp_xor = h.tagged_fp_xor;
+    return 0;
+}
+
+int vsr_expand_shape(const VsrModel* m, int* warps, int* blocks, int* passes, int* stage_rows) {
+    if (!m || !m->gpu) return VSR_RC_CONFIG_ERROR;
+    *warps = m->gpu->warps;
+    *blocks = m->gpu->blocks;
+    *passes = m->gpu->passes;
+    *stage_rows = m->gpu->stage_rows;
+    return 0;
+}
+
 int vsr_engine_reset(VsrEngine* e) {
     CK(cudaMemsetAsync(e->table, 0, e->table_cap * 16, e->stream));
     const uint64_t tc = e->st.table_capacity, fc = e->st.frontier_capacity, bt = e->st.bytes_table, bf = e->st.bytes_frontier;

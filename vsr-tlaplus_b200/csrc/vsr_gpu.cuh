@@ -1063,6 +1063,68 @@ static __global__ void lookup_kernel(const uint64_t* table, unsigned long long c
     *meta_out = 0;
 }
 
+/* per-level audit (tests, vsr_engine_audit_level): seen-set entries tagged with a level, and the level's frontier looked up
+   in the seen-set with the insert's probe order (entry by entry from the home bucket; the first empty slot ends the chain),
+   plus order-independent digests of the frontier and of the tagged entries' fingerprints */
+struct AuditSums {
+    unsigned long long tagged, found, fp_sum, fp_xor, words_sum, words_xor, tagged_fp_sum, tagged_fp_xor;
+};
+__device__ __forceinline__ void audit_add(unsigned long long* dst, unsigned long long v, bool is_xor) {
+    for (int o = 16; o; o >>= 1) v = is_xor ? v ^ __shfl_xor_sync(0xffffffffu, v, o) : v + __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) {
+        if (is_xor) atomicXor(dst, v);
+        else atomicAdd(dst, v);
+    }
+}
+static __global__ void audit_table_kernel(const uint64_t* table, unsigned long long cap, int level, AuditSums* out) {
+    unsigned long long n = 0, fs = 0, fx = 0;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const uint64_t e0 = table[2 * i];
+        if (e0 != 0 && (int)(table[2 * i + 1] >> 56) == level) {
+            n++;
+            fs += mix64(e0);
+            fx ^= mix64(e0);
+        }
+    }
+    audit_add(&out->tagged, n, false);
+    audit_add(&out->tagged_fp_sum, fs, false);
+    audit_add(&out->tagged_fp_xor, fx, true);
+}
+template <class L> __global__ void audit_frontier_kernel(const ExpandParams P, unsigned long long n_states, AuditSums* out) {
+    unsigned long long found = 0, fs = 0, fx = 0, ws = 0, wx = 0;
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_states; i += (unsigned long long)gridDim.x * blockDim.x) {
+        uint32_t w[L::NW];
+        const uint32_t* st = out_state<L::NW>(P, i);
+        uint64_t hw = 0;
+        for (int j = 0; j < L::NW; j++) {
+            w[j] = st[j];
+            hw = mix64(hw ^ ((uint64_t)j << 32 | w[j]));
+        }
+        uint64_t fp = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
+        if (fp == 0) fp = 1;
+        const uint32_t chk = check_hash<L>(w, P.run.use_view != 0);
+        unsigned long long h = table_home(P.table_cap, fp);
+        for (unsigned long long k = 0; k < P.table_cap; k++) {
+            const uint64_t e0 = P.table[2 * h], e1 = P.table[2 * h + 1];
+            if (e0 == 0) break;
+            if (e0 == fp && (uint32_t)e1 == chk) {
+                found += (int)(e1 >> 56) == P.level;
+                break;
+            }
+            if (++h >= P.table_cap) h = 0;
+        }
+        fs += mix64(fp);
+        fx ^= mix64(fp);
+        ws += hw;
+        wx ^= hw;
+    }
+    audit_add(&out->found, found, false);
+    audit_add(&out->fp_sum, fs, false);
+    audit_add(&out->fp_xor, fx, true);
+    audit_add(&out->words_sum, ws, false);
+    audit_add(&out->words_xor, wx, true);
+}
+
 /* ------------------------------------------------------------------ simulation mode (TLC `-simulate`)
    One thread per random walk from Init, `depth` states long at most; the invariant is checked on every state reached.
    The first violating (walk, depth) is kept (smallest walk index wins) and re-walked on the host for the trace. */

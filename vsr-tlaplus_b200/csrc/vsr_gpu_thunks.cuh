@@ -21,6 +21,9 @@ struct GpuOps {
     int tie_bytes;
     cudaError_t (*prepare)(int* blocks_per_sm);
     cudaError_t (*launch_simulate)(const SimParams&, int grid, cudaStream_t);
+    /* the expand kernel's shape (ExpandCfg): warps per block, blocks per SM, scan passes per round, staging rows per warp */
+    int warps, blocks, passes, stage_rows;
+    cudaError_t (*launch_audit)(const ExpandParams&, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t);
 };
 
 /* what a layout plug-in must have been compiled against: the version constant AND the shapes of the structs the kernels and the
@@ -60,10 +63,17 @@ template <class L> struct GpuThunks {
         simulate_kernel<L><<<grid, 128, 0, st>>>(q);
         return cudaGetLastError();
     }
+    static cudaError_t launch_audit(const ExpandParams& p, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t st) {
+        audit_table_kernel<<<sms * 8, 256, 0, st>>>(p.table, p.table_cap, p.level, out);
+        if (n_states) audit_frontier_kernel<L><<<sms * 8, 256, 0, st>>>(p, n_states, out);
+        return cudaGetLastError();
+    }
     static uint32_t chk(const uint32_t* w, int use_view) { return check_hash<L>(w, use_view != 0); }
     static const GpuOps* get() {
-        static const GpuOps ops = {chk, L::R, L::V, L::K, L::NW, L::BYTES, (int)(L::BYTES + sizeof(RecHdr)), sizeof(typename ExpandCfg<L>::Smem), ExpandCfg<L>::WARPS * 32,
-                                   launch_expand, launch_insert, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate};
+        typedef ExpandCfg<L> Cfg;
+        static const GpuOps ops = {chk, L::R, L::V, L::K, L::NW, L::BYTES, (int)(L::BYTES + sizeof(RecHdr)), sizeof(typename Cfg::Smem), Cfg::WARPS * 32,
+                                   launch_expand, launch_insert, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate,
+                                   Cfg::WARPS, Cfg::BLOCKS, Cfg::PASSES, Expander<L, false>::SROWS, launch_audit};
         return &ops;
     }
 };

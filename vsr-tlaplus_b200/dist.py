@@ -255,6 +255,12 @@ class GpuEngine:
         self._ck(self.lib.vsr_engine_lookup(self._e, buf, C.byref(lvl), C.byref(owner)))
         return int(lvl.value), int(owner.value)
 
+    def audit(self) -> "ck.VsrLevelAudit":
+        """audit of the level just finished: seen-set entries tagged with it, its states found there, frontier digests"""
+        a = ck.VsrLevelAudit()
+        self._ck(self.lib.vsr_engine_audit_level(self._e, C.byref(a)))
+        return a
+
     def collected(self, level: int) -> bytes:
         n = int(self.lib.vsr_engine_collected(self._e, level, None, 0))
         buf = (C.c_uint8 * max(n * self.mc.state_bytes, 1))()
