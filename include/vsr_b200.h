@@ -159,13 +159,14 @@ typedef struct VsrStats {
 
 typedef struct VsrEngine VsrEngine;
 
-/* One-call BFS on one GPU.  Fails loudly (153) when no CUDA device is usable — there is no CPU
- * fallback.  If trace_out != NULL and a violation/deadlock is found, writes the counterexample
- * (packed states, trace_cap capacity) with its action ids; stats.trace_len is its length. */
+/* One-call BFS on one GPU: engine creation (stats.seconds_setup), vsr_bfs_sharded on that world-1 engine, teardown.
+ * Fails loudly (153) when no CUDA device is usable — there is no CPU fallback.  If trace_out != NULL and a
+ * violation/deadlock is found, writes the counterexample (packed states, trace_cap capacity) with its action ids;
+ * stats.trace_len is its length, stats.violation_mask the invariants its last state violates. */
 int vsr_bfs(const VsrModel* m, const VsrRunOpts* opts, VsrStats* stats, void* trace_out, uint8_t* trace_actions,
             size_t trace_cap);
 
-/* Stepwise engine (what vsr_bfs and vsr_bfs_sharded are made of).
+/* Stepwise engine (what vsr_bfs_sharded, and through it vsr_bfs and vsr_bfs_multi, is made of).
  * rank/world: this engine owns the fingerprints f with owner(f) == rank (world = 1, 2, 4 or 8: the high bits of f). */
 int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int world, VsrEngine** out, char* err,
                       size_t errcap);
@@ -209,7 +210,7 @@ int vsr_engine_lookup(VsrEngine* e, const void* state, int* level_out, int* owne
  * current frontier, every seen-set entry {fingerprint, meta}, the trace records and the run's statistics, to one file.
  * vsr_engine_recover loads it into a fresh (or reset) engine of the same model, rank and world; the seen-set is re-inserted
  * entry by entry, so its capacity may differ from the one the checkpoint was written with.  `totals` (may be NULL) travels
- * with the file: vsr_bfs / vsr_bfs_sharded store the job's running totals there.  150 = not a checkpoint of this model. */
+ * with the file: vsr_bfs_sharded stores the job's running totals there.  150 = not a checkpoint of this model. */
 int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals);
 int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out);
 /* forget everything explored (clears the seen-set, keeps the allocations): ready for seed_init again */
@@ -233,7 +234,8 @@ int vsr_engine_audit_level(VsrEngine* e, VsrLevelAudit* out);
 /* the expand kernel's shape for this model's layout (no GPU needed): warps per block, blocks per SM, scan passes per
  * round, staging rows per warp */
 int vsr_expand_shape(const VsrModel* m, int* warps, int* blocks, int* passes, int* stage_rows);
-/* Rebuild the counterexample ending at local state id (single-rank engines). */
+/* Rebuild the behaviour from Init to local state id (world-1 engines; tests): the parent-chain walk of vsr_bfs_sharded,
+ * replayed with vsr_replay_candidates.  Returns the number of states, or a negative status. */
 int vsr_engine_build_trace(VsrEngine* e, uint64_t local_id, void* trace_out, uint8_t* trace_actions, size_t trace_cap);
 
 /* ---- several GPUs of one node (SURVEY §8e: TLC's `-workers` / distributed mode).  One rank per GPU — processes
@@ -265,7 +267,8 @@ int vsr_engine_attach_group(VsrEngine* e, VsrGroup* g, uint64_t inbox_records);
 int vsr_engine_attach_staged(VsrEngine* e, uint64_t inbox_records, void** stage_out, void** inbox_out, uint64_t* cap_out);
 int vsr_engine_detach(VsrEngine* e);                                 /* collective when attached to a group */
 uint64_t vsr_engine_default_inbox_records(const VsrEngine* e);
-/* The whole BFS, called by every rank of the group with the same opts; all ranks return the same rc and the same totals
+/* The whole BFS, called by every rank of the group with the same opts (world 1: one call, no group); it starts from Init,
+ * or from opts.recover_path, whatever the engine explored before.  All ranks return the same rc and the same totals
  * (records_sent / received, bytes_* and kernel_launches are this rank's).  part_states = frontier states per rank and step
  * (0 = from the inbox size).  On a violation / deadlock trace_cands[0 .. *trace_len) is the candidate chain from Init,
  * walked across ranks: vsr_replay_candidates turns it into the literal behaviour. */

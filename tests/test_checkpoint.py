@@ -38,6 +38,29 @@ def test_recovered_run_equals_uninterrupted_run(pkg, tmp_path):
     same_exploration(mc.check(stop_on_violation=False, recover_path=ck2, table_capacity=1 << 21, frontier_capacity=1 << 18), whole)
 
 
+def test_collecting_check_and_one_rank_engine_checkpoint_to_the_given_path(pkg, tmp_path):
+    """check(collect_levels=True) writes and continues from checkpoints as check() does, and one rank writes <path> itself,
+    not <path>.rank0"""
+    from vsr_tlaplus_b200 import dist as vdist
+    mc = pkg.ModelChecker.from_constants(3, 2, 1, symmetry=False)
+    caps = dict(table_capacity=1 << 21, frontier_capacity=1 << 18)
+    whole = mc.check(stop_on_violation=False, **caps)
+    ck = str(tmp_path / "collect.ckpt")
+    part = mc.check(collect_levels=True, stop_on_violation=False, max_depth=17, checkpoint_path=ck, checkpoint_seconds=1e9, **caps)
+    assert part.depth == 17 and os.path.exists(ck)
+    rest = mc.check(collect_levels=True, stop_on_violation=False, recover_path=ck, **caps)
+    same_exploration(rest, whole)
+    assert [len(lv) // mc.state_bytes for lv in rest.levels] == [0] * 17 + whole.level_sizes[17:]
+    eng = vdist.GpuEngine(mc, 0, 1, **caps)
+    ck1 = str(tmp_path / "engine.ckpt")
+    try:
+        assert eng.run(stop_on_violation=False, max_depth=17, checkpoint_path=ck1, checkpoint_seconds=1e9).depth == 17
+    finally:
+        eng.close()
+    assert os.path.exists(ck1) and not os.path.exists(ck1 + ".rank0")
+    same_exploration(mc.check(stop_on_violation=False, recover_path=ck1, **caps), whole)
+
+
 def test_counterexample_after_recovery_is_a_behaviour(pkg, tmp_path):
     """The trace records travel with the checkpoint: a violation found after recovery is traced back to Init through states
     explored before it.  Every step must be a step of Next, the last state (only) violates the invariant; the oracle finds the

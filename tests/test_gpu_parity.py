@@ -137,6 +137,40 @@ def test_counterexample_is_a_behaviour(pkg):
         assert L.orc_invariant_flat(q, C.byref(f)) == 1
 
 
+@pytest.mark.parametrize("stop", [True, False])
+def test_one_gpu_paths_agree(pkg, stop):
+    """check() (vsr_bfs), check(collect_levels=True) and GpuEngine(mc, 0, 1).run() run the one level loop: the same verdict,
+    totals, per-level tables and launches, whether the run stops at the violation or continues past it.  Which violating
+    state a run reports, and which parent each state keeps, follow the order in which warps insert states, so the three
+    counterexamples are compared as behaviours: as long as the BFS depth, every step a step of Next, only the last state
+    violating."""
+    from vsr_tlaplus_b200 import dist as vdist
+    inv = ("AcknowledgedWritesExistOnMajority",)
+    mc = pkg.ModelChecker.from_constants(3, 2, 1, invariants=inv)
+    caps = dict(table_capacity=1 << 21, frontier_capacity=1 << 18)
+    one = mc.check(stop_on_violation=stop, **caps)
+    col = mc.check(stop_on_violation=stop, collect_levels=True, **caps)
+    eng = vdist.GpuEngine(mc, 0, 1, **caps)
+    try:
+        run = eng.run(stop_on_violation=stop)
+    finally:
+        eng.close()
+    k = len(run.level_generated)  # levels expanded
+    assert run.rc == 12 and run.violation_level > 8 and run.complete == (not stop) and len(run.level_ms) == k
+    lit = pkg.ModelChecker.from_constants(3, 2, 1, symmetry=False, invariants=inv)
+    for r in (one, col):
+        assert (r.rc, r.generated, r.distinct, r.queue, r.depth, r.complete) == (run.rc, run.generated, run.distinct, run.queue, run.depth, run.complete)
+        assert r.level_sizes == run.level_sizes
+        assert r.level_generated[:k] == run.level_generated and not any(r.level_generated[k:]) and not any(r.level_ms[k:])
+        assert (r.violation_level, r.h2_ties, r.kernel_launches) == (run.violation_level, run.h2_ties, run.launches)
+        assert r.violated_invariants == list(inv)
+    for trace in (one.trace, col.trace, vdist.replay_trace(mc, run.trace_cands)):
+        assert len(trace) == run.violation_level and trace[0] == ("Initial predicate", lit.init_state())
+        for (_, a), (act, b) in zip(trace, trace[1:]):
+            assert (b, act) in [(t, pkg.ACTION_NAMES[x]) for t, x, _ in lit.successors(a)]
+        assert [lit.invariant(s) != 0 for _, s in trace] == [False] * (len(trace) - 1) + [True]
+
+
 def test_frontier_overflow_is_loud(pkg):
     mc = pkg.ModelChecker.from_constants(3, 2, 2)
     res = mc.check(max_depth=12, table_capacity=1 << 20, frontier_capacity=256)

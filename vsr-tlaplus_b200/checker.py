@@ -505,11 +505,11 @@ class ModelChecker:
             trace=trace or [], levels=levels or [])
 
     def check(self, **kw) -> CheckResult:
-        """One-GPU BFS through the single C-ABI call ``vsr_bfs`` (counterexample included)."""
-        collect = kw.get("collect_levels", False)
-        if collect:
-            return self._check_stepwise(**kw)
+        """One-GPU BFS through the single C-ABI call ``vsr_bfs`` (counterexample included).  With collect_levels=True the
+        same level loop, ``vsr_bfs_sharded``, runs on an engine held here, so that every level's states can be read back."""
         o = self.run_opts(**kw)
+        if o.collect_levels:
+            return self._check_collecting(o)
         st = VsrStats()
         cap = 512
         tr = self._buf(cap)
@@ -573,66 +573,31 @@ class ModelChecker:
         n = self._lib.vsr_walk(self._h, seed, walk, depth, cands, C.byref(va))
         return [int(cands[i]) for i in range(n)], int(va.value)
 
-    def _check_stepwise(self, **kw) -> CheckResult:
-        """Same BFS pumped level by level through the engine entry points (keeps every level for tests)."""
-        import time
-        o = self.run_opts(**kw)
+    def _check_collecting(self, o: VsrRunOpts) -> CheckResult:
+        """``check(collect_levels=True)``: vsr_bfs_sharded on a world-1 engine, then every level's states read back."""
         lib = self._lib
         e = C.c_void_p()
         err = C.create_string_buffer(512)
         rc = lib.vsr_engine_create(self._h, C.byref(o), 0, 1, C.byref(e), err, len(err))
         if rc:
             raise VsrError(rc, err.value.decode())
-        t0 = time.time()
         try:
-            li = VsrLevelInfo()
-            result, complete, bad = 0, False, None
-            rc = lib.vsr_engine_seed_init(e) or lib.vsr_engine_finish_level(e, C.byref(li))
-            level = 1
-            while not rc:
-                if li.error_code:
-                    result = 255
-                    break
-                if li.overflow:
-                    result = 152
-                    break
-                if li.violation:
-                    result, bad = 12, int(li.violation_id)
-                    if o.stop_on_violation:
-                        break
-                if li.deadlock:
-                    result, bad = 11, int(li.deadlock_id)
-                    break
-                if lib.vsr_engine_frontier_size(e) == 0:
-                    complete = True
-                    break
-                if o.max_depth and level >= o.max_depth:
-                    break
-                rc = lib.vsr_engine_expand(e) or lib.vsr_engine_finish_level(e, C.byref(li))
-                level += 1
-            if rc:
-                raise VsrError(rc, lib.vsr_engine_last_error(e).decode())
             st = VsrStats()
-            lib.vsr_engine_stats(e, C.byref(st))
-            st.depth = st.num_levels
-            st.complete = int(complete)
-            st.queue = 0 if complete else lib.vsr_engine_frontier_size(e)
-            st.seconds_total = time.time() - t0
+            cap = 4096
+            cands, n = (C.c_uint32 * cap)(), C.c_int(0)
+            rc = lib.vsr_bfs_sharded(e, C.byref(o), 0, C.byref(st), cands, C.byref(n), cap)
+            if rc == 153:
+                raise VsrError(rc, lib.vsr_engine_last_error(e).decode())
             levels = []
             sb = self.state_bytes
             for lv in range(1, int(st.num_levels) + 1):
-                n = lib.vsr_engine_collected(e, lv, None, 0)
-                buf = (C.c_uint8 * (n * sb))()
-                lib.vsr_engine_collected(e, lv, buf, n)
+                k = lib.vsr_engine_collected(e, lv, None, 0)
+                buf = (C.c_uint8 * (k * sb))()
+                lib.vsr_engine_collected(e, lv, buf, k)
                 levels.append(bytes(buf))
-            trace = []
-            if bad is not None and o.keep_trace:
-                cap = 512
-                tr = self._buf(cap)
-                acts = (C.c_uint8 * cap)()
-                n = lib.vsr_engine_build_trace(e, bad, tr, acts, cap)
-                raw = bytes(tr)
-                trace = [(ACTION_NAMES[acts[i]], raw[i * sb:(i + 1) * sb]) for i in range(max(n, 0))]
-            return self.result_from_stats(st, result, trace, levels)
+            trace = self._trace_from_cands(cands, n.value) if st.trace_len else []
+            if rc == 12 and trace:
+                st.violation_mask = self.invariant(trace[-1][1])
+            return self.result_from_stats(st, rc, trace, levels)
         finally:
             lib.vsr_engine_destroy(e)

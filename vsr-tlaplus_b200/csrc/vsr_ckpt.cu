@@ -241,6 +241,7 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
     }
     int rc = vsr_engine_reset(e);
     if (rc) return rc;
+    e->touched = true; /* from here on a failure leaves part of the checkpoint in the engine */
     CK(cudaStreamSynchronize(e->stream));
     std::vector<uint8_t> host;
     /* 1. the frontier, into buffer 0 */
@@ -295,6 +296,7 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
     e->n_cur = h.n_cur; e->cur_base = h.cur_base; e->next_base = h.next_base;
     e->level = h.level;
     e->level_open = false;
+    if (e->opts.collect_levels) e->collected.resize(h.level); /* depths up to the checkpoint's were collected by another run: empty */
     e->records_sent = h.records_sent; e->records_received = h.records_received;
     if (totals_out) *totals_out = tot;
     return 0;

@@ -1,8 +1,8 @@
 /*
- * vsr_gpu.cu — host driver of the BFS wavefront and the GPU half of the C ABI
- * (vsr_bfs, vsr_engine_*; include/vsr_b200.h).  "Thin C++ driver that pumps wavefronts":
- * per level one expand launch (plus insert launches for records received from peer ranks),
- * one small counter read-back, swap frontiers.  Kernels: vsr_gpu.cuh.
+ * vsr_gpu.cu — the engine primitives of the GPU half of the C ABI (vsr_engine_*; include/vsr_b200.h): create, seed Init,
+ * one launch of the wavefront kernel (expand a part of the frontier, insert records received from peer ranks), finish a
+ * level (one small counter read-back, swap frontiers), reset; plus vsr_simulate and vsr_probe_bench.  The level loop that
+ * pumps them is vsr_bfs_sharded (vsr_shard.cu), for one GPU as for several.  Kernels: vsr_gpu.cuh.
  * There is NO CPU fallback: without a usable CUDA device every entry point returns 153.
  */
 #include <stddef.h>
@@ -37,6 +37,7 @@ int engine_reset_level(VsrEngine* e) {
     CK(cudaMemcpyAsync(&e->ctr->viol_id, &ones, 8, cudaMemcpyHostToDevice, e->stream));
     CK(cudaMemcpyAsync(&e->ctr->dead_id, &ones, 8, cudaMemcpyHostToDevice, e->stream));
     e->level_open = true;
+    e->touched = true;
     e->level_ms_acc = 0;
     e->level_ms_insert_acc = 0;
     return 0;
@@ -510,6 +511,8 @@ int vsr_expand_shape(const VsrModel* m, int* warps, int* blocks, int* passes, in
 }
 
 int vsr_engine_reset(VsrEngine* e) {
+    if (!e->touched) return 0; /* as created or last reset: clearing tens of GB again would only cost time */
+    e->touched = false;
     CK(cudaMemsetAsync(e->table, 0, e->table_cap * 16, e->stream));
     const uint64_t tc = e->st.table_capacity, fc = e->st.frontier_capacity, bt = e->st.bytes_table, bf = e->st.bytes_frontier;
     memset(&e->st, 0, sizeof e->st);
@@ -534,95 +537,6 @@ uint64_t vsr_engine_collected(const VsrEngine* e, int level, void* host_out, uin
     const uint64_t n = v.size() / e->g->bytes;
     if (host_out && cap_states >= n) memcpy(host_out, v.data(), v.size());
     return n;
-}
-
-int vsr_engine_build_trace(VsrEngine* e, uint64_t local_id, void* trace_out, uint8_t* trace_actions, size_t trace_cap) {
-    if (e->world != 1) return -VSR_RC_ERROR; /* multi-rank chains are walked by the host that owns the collectives */
-    std::vector<uint32_t> cands;
-    uint64_t id = local_id;
-    const uint64_t root_parent = ROOT_GID;
-    for (int guard = 0; guard < 100000; guard++) {
-        uint64_t parent;
-        uint32_t cand;
-        if (vsr_engine_trace_record(e, id, &parent, &cand)) return -VSR_RC_ERROR;
-        if (parent == root_parent) break; /* Init */
-        cands.push_back(cand);
-        id = parent & ((1ull << 40) - 1);
-    }
-    std::vector<uint32_t> fwd(cands.rbegin(), cands.rend());
-    return vsr_replay_candidates(e->m, fwd.data(), (int)fwd.size(), trace_out, trace_actions, trace_cap);
-}
-
-int vsr_bfs(const VsrModel* m, const VsrRunOpts* opts, VsrStats* stats, void* trace_out, uint8_t* trace_actions, size_t trace_cap) {
-    if (!m || !opts || !stats) return VSR_RC_ERROR;
-    const double t0 = now_s();
-    VsrEngine* e = nullptr;
-    char err[256];
-    int rc = vsr_engine_create(m, opts, 0, 1, &e, err, sizeof err);
-    if (rc) {
-        memset(stats, 0, sizeof *stats);
-        stats->rc = rc;
-        if (opts->verbose) fprintf(stderr, "vsr_bfs: %s\n", err);
-        return rc;
-    }
-    const double t_setup = now_s() - t0;
-    VsrLevelInfo li;
-    memset(&li, 0, sizeof li);
-    int result = 0;
-    bool complete = false, bounded = false;
-    uint64_t bad_id = ~0ull;
-    if (opts->recover_path) { /* TLC -recover: continue from a checkpoint instead of Init */
-        rc = vsr_engine_recover(e, opts->recover_path, nullptr);
-        if (!rc && e->st.violation_level) { result = VSR_RC_VIOLATION; bad_id = e->st.violation_id; } /* found before the checkpoint, run continued past it */
-    } else {
-        rc = vsr_engine_seed_init(e);
-        if (!rc) rc = vsr_engine_finish_level(e, &li);
-    }
-    double last_ckpt = now_s();
-    while (!rc) {
-        if (li.error_code) { result = VSR_RC_ERROR; break; }
-        if (li.overflow) { result = VSR_RC_TOO_LARGE; break; }
-        if (li.violation && opts->stop_on_violation) { result = VSR_RC_VIOLATION; bad_id = li.violation_id; break; }
-        if (li.violation && !result) { result = VSR_RC_VIOLATION; bad_id = li.violation_id; }
-        if (li.deadlock) { result = VSR_RC_DEADLOCK; bad_id = li.deadlock_id; break; }
-        if (e->n_cur == 0) { complete = true; break; }
-        if (opts->max_depth && e->level >= opts->max_depth) { bounded = true; break; }
-        if (opts->max_states && e->st.distinct >= opts->max_states) { bounded = true; break; }
-        if (opts->max_seconds > 0 && now_s() - t0 >= opts->max_seconds) { bounded = true; break; }
-        if (e->level >= 254) { result = VSR_RC_TOO_LARGE; break; } /* 8-bit level tag in the seen-set */
-        if (opts->checkpoint_path && now_s() - last_ckpt >= opts->checkpoint_seconds) { /* TLC -checkpoint: at a level boundary */
-            rc = vsr_engine_checkpoint(e, opts->checkpoint_path, nullptr);
-            if (rc) break;
-            last_ckpt = now_s();
-            if (opts->verbose) fprintf(stderr, "Checkpointing of run %s completed (depth %d, %llu distinct states).\n", opts->checkpoint_path, e->level, (unsigned long long)e->st.distinct);
-        }
-        rc = vsr_engine_expand(e);
-        if (rc) break;
-        rc = vsr_engine_finish_level(e, &li);
-        if (opts->verbose && !rc)
-            fprintf(stderr, "depth %3d: %12llu new  %12llu generated  %8.3f ms\n", e->level, (unsigned long long)li.new_states,
-                    (unsigned long long)li.generated, li.ms);
-    }
-    /* a run that stops on a bound (-depth, max_states, max_seconds) leaves a checkpoint to continue from */
-    if (!rc && bounded && opts->checkpoint_path) rc = vsr_engine_checkpoint(e, opts->checkpoint_path, nullptr);
-    if (rc) result = rc;
-    VsrStats s = e->st;
-    s.rc = result;
-    s.complete = complete ? 1 : 0;
-    s.depth = s.num_levels;
-    s.queue = complete ? 0 : e->n_cur;
-    if (bad_id != ~0ull && trace_out && e->trace) {
-        int n = vsr_engine_build_trace(e, bad_id, trace_out, trace_actions, trace_cap);
-        s.trace_len = n > 0 ? n : 0;
-        if (n > 0 && result == VSR_RC_VIOLATION)
-            s.violation_mask = m->ops->invariant(&m->run, (const uint32_t*)((const uint8_t*)trace_out + (size_t)(n - 1) * m->ops->bytes));
-    }
-    s.seconds_total = now_s() - t0;
-    s.seconds_setup = t_setup;
-    *stats = s;
-    if (rc && opts->verbose) fprintf(stderr, "vsr_bfs: %s\n", e->last_error);
-    vsr_engine_destroy(e);
-    return result;
 }
 
 /* TLC `-simulate`: random walks on the GPU; a violating walk is re-walked on the host (same generator, same step

@@ -1,6 +1,7 @@
 /*
- * vsr_shard.cu — the BFS on several GPUs of one node (SURVEY §8e): the reachable set is sharded by the high bits of the
- * 64-bit fingerprint, every rank (one per GPU) owns its shard of the seen-set, of the frontier and of the trace.
+ * vsr_shard.cu — the BFS's level loop, on one GPU or on several GPUs of one node (SURVEY §8e): the reachable set is sharded
+ * by the high bits of the 64-bit fingerprint, every rank (one per GPU) owns its shard of the seen-set, of the frontier and of
+ * the trace.  One GPU is world 1: one launch per level, no group, no inbox.
  *
  * The exchange is fused into the wavefront kernel: a successor owned by another rank is stored by expand_kernel straight
  * into that rank's inbox over NVLink (the inbox is mapped into this process with CUDA IPC, or is a peer pointer when the
@@ -14,6 +15,7 @@
  *   vsr_engine_attach_staged  the same kernel writing into a LOCAL staging buffer, for a host that moves the records with
  *                             a collective instead (dist.ShardedBfs over torch.distributed: NCCL all-to-all, or gloo in tests)
  *   vsr_bfs_sharded           the level loop, called by every rank; all ranks return the same totals
+ *   vsr_bfs                   one GPU: a world-1 engine through vsr_bfs_sharded
  *   vsr_bfs_multi             one process, one thread per GPU (vsrmc -gpus N)
  */
 #include <stdlib.h>
@@ -59,6 +61,47 @@ struct WalkMsg {
 int set_error(VsrEngine* e, const char* fmt, const char* a = "") {
     snprintf(e->last_error, sizeof e->last_error, fmt, a);
     return VSR_RC_SYSTEM;
+}
+
+/* The candidate chain from Init to state `gid` (rank << 40 | local id), from the (parent, candidate) trace records.  With
+   several ranks the owner of each record shares it in an all-gather: every rank calls this with the same gid. */
+int walk_trace(VsrEngine* e, uint64_t gid, std::vector<uint32_t>& cands) {
+    cands.clear();
+    for (int guard = 0; guard < 4096; guard++) {
+        const int owner = (int)(gid >> 40);
+        WalkMsg wm, wms[MAX_WORLD];
+        memset(&wm, 0, sizeof wm);
+        if (owner == e->rank) {
+            uint64_t parent = 0;
+            uint32_t cand = 0;
+            wm.ok = vsr_engine_trace_record(e, gid & ((1ull << 40) - 1), &parent, &cand) == 0;
+            wm.parent = parent;
+            wm.cand = cand;
+        }
+        if (e->world > 1) {
+            if (vsr_group_allgather(e->group, &wm, sizeof wm, wms)) return set_error(e, "%s", e->group->last_error);
+            wm = wms[owner < e->world ? owner : 0];
+        }
+        if (!wm.ok) {
+            snprintf(e->last_error, sizeof e->last_error, "trace record of state %llu cannot be read", (unsigned long long)gid);
+            return VSR_RC_ERROR;
+        }
+        if (wm.parent == ROOT_GID) break;
+        cands.push_back(wm.cand);
+        gid = wm.parent;
+    }
+    std::reverse(cands.begin(), cands.end());
+    return 0;
+}
+
+/* The counterexample of the one-call APIs: the candidate chain vsr_bfs_sharded walked (stats->trace_len > 0: it did)
+   replayed into literal states; a violation reports the invariants its last state violates. */
+void replay_counterexample(const VsrModel* m, int rc, const uint32_t* cands, int n_cands, VsrStats* stats, void* trace_out, uint8_t* trace_actions,
+                           size_t trace_cap) {
+    const int n = trace_out && stats->trace_len > 0 ? vsr_replay_candidates(m, cands, n_cands, trace_out, trace_actions, trace_cap) : 0;
+    stats->trace_len = n > 0 ? n : 0;
+    if (n > 0 && rc == VSR_RC_VIOLATION)
+        stats->violation_mask = m->ops->invariant(&m->run, (const uint32_t*)((const uint8_t*)trace_out + (size_t)(n - 1) * m->ops->bytes));
 }
 
 } // namespace
@@ -205,13 +248,16 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     bool complete = false, bounded = false;
     uint64_t bad_gid = ~0ull;
     double kernel_ms = 0, insert_ms = 0;
-    /* checkpoints: every rank writes / reads <path>.rank<r> at the same level boundary (rank 0's clock decides when) */
-    const std::string ckpt_path = opts->checkpoint_path ? std::string(opts->checkpoint_path) + ".rank" + std::to_string(me) : std::string();
+    /* checkpoints: with several ranks every rank writes / reads <path>.rank<r> at the same level boundary (rank 0's clock
+       decides when); one rank uses <path> itself */
+    auto rank_file = [&](const char* path) { return W > 1 ? std::string(path) + ".rank" + std::to_string(me) : std::string(path); };
+    const std::string ckpt_path = opts->checkpoint_path ? rank_file(opts->checkpoint_path) : std::string();
+    const std::string slowest = W > 1 ? " (slowest of " + std::to_string(W) + " GPUs)" : "";
     double last_ckpt = now_s();
     bool resumed = false;
     int rc;
     if (opts->recover_path) {
-        rc = vsr_engine_recover(e, (std::string(opts->recover_path) + ".rank" + std::to_string(me)).c_str(), &tot);
+        rc = vsr_engine_recover(e, rank_file(opts->recover_path).c_str(), &tot);
         if (!rc) {
             resumed = true;
             level = e->level - 1; /* the loop's first pass stands at the checkpoint's level boundary without finishing a level */
@@ -281,7 +327,7 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
             tot.num_levels = level;
         }
         if (opts->verbose && me == 0 && level >= 2 && !boundary_only)
-            fprintf(stderr, "depth %3d: %12llu new  %12llu generated  %8.3f ms (slowest of %d GPUs)\n", level, (unsigned long long)n_new, (unsigned long long)n_gen, ms, W);
+            fprintf(stderr, "depth %3d: %12llu new  %12llu generated  %8.3f ms%s\n", level, (unsigned long long)n_new, (unsigned long long)n_gen, ms, slowest.c_str());
         if (err) { result = VSR_RC_ERROR; tot.error_code = err; break; }
         if (ovf) { result = VSR_RC_TOO_LARGE; break; }
         if (viol && !tot.violation_level) {
@@ -303,7 +349,8 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
             step_rc = vsr_engine_checkpoint(e, ckpt_path.c_str(), &tot); /* a failure travels to everybody in the next all-gather */
             last_ckpt = now_s();
             if (opts->verbose && me == 0 && !step_rc)
-                fprintf(stderr, "Checkpointing of run %s.rank* completed (depth %d, %llu distinct states).\n", opts->checkpoint_path, level, (unsigned long long)tot.distinct);
+                fprintf(stderr, "Checkpointing of run %s%s completed (depth %d, %llu distinct states).\n", opts->checkpoint_path, W > 1 ? ".rank*" : "", level,
+                        (unsigned long long)tot.distinct);
         }
         /* ---- the next level, in steps: step k expands part k and pushes into inbox half k & 1, and drains what the
            peers pushed here in step k - 1; one more launch drains the last part's records */
@@ -392,28 +439,7 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     /* counterexample: follow (parent, candidate) records across ranks back to Init */
     if (bad_gid != ~0ull && trace_cands && e->trace && opts->keep_trace) {
         std::vector<uint32_t> cands;
-        uint64_t gid = bad_gid;
-        for (int guard = 0; guard < 4096; guard++) {
-            const int owner = (int)(gid >> 40);
-            WalkMsg wm, wms[MAX_WORLD];
-            memset(&wm, 0, sizeof wm);
-            if (owner == me) {
-                uint64_t parent = 0;
-                uint32_t cand = 0;
-                wm.ok = vsr_engine_trace_record(e, gid & ((1ull << 40) - 1), &parent, &cand) == 0;
-                wm.parent = parent;
-                wm.cand = cand;
-            }
-            if (W > 1) {
-                if (vsr_group_allgather(g, &wm, sizeof wm, wms)) return set_error(e, "%s", g->last_error);
-                wm = wms[owner < W ? owner : 0];
-            }
-            if (!wm.ok) break;
-            if (wm.parent == ROOT_GID) break;
-            cands.push_back(wm.cand);
-            gid = wm.parent;
-        }
-        std::reverse(cands.begin(), cands.end());
+        if ((rc = walk_trace(e, bad_gid, cands))) return rc;
         const size_t n = std::min(cands.size(), trace_cap);
         memcpy(trace_cands, cands.data(), n * sizeof(uint32_t));
         if (trace_len) *trace_len = (int)n;
@@ -493,14 +519,42 @@ int vsr_bfs_multi(const VsrModel* m, const VsrRunOpts* opts, int ngpus, uint64_t
             if (!errors[r].empty()) { snprintf(err, errcap, "GPU %d: %s", opts->device + r, errors[r].c_str()); break; }
     }
     *stats = st[0];
-    if ((rc == VSR_RC_VIOLATION || rc == VSR_RC_DEADLOCK || (rc == 0 && st[0].violation_level)) && trace_out && lens[0] >= 0 && st[0].trace_len > 0) {
-        const int n = vsr_replay_candidates(m, cands[0].data(), lens[0], trace_out, trace_actions, trace_cap);
-        stats->trace_len = n > 0 ? n : 0;
-        if (n > 0 && stats->violation_level)
-            stats->violation_mask = m->ops->invariant(&m->run, (const uint32_t*)((const uint8_t*)trace_out + (size_t)(n - 1) * m->ops->bytes));
-    } else stats->trace_len = 0;
+    replay_counterexample(m, rc, cands[0].data(), lens[0], stats, trace_out, trace_actions, trace_cap);
     stats->seconds_total = now_s() - t0;
     return rc;
+}
+
+/* One GPU: the same level loop on a world-1 engine (one launch per level) */
+int vsr_bfs(const VsrModel* m, const VsrRunOpts* opts, VsrStats* stats, void* trace_out, uint8_t* trace_actions, size_t trace_cap) {
+    if (!m || !opts || !stats) return VSR_RC_ERROR;
+    memset(stats, 0, sizeof *stats);
+    const double t0 = now_s();
+    VsrEngine* e = nullptr;
+    char err[256];
+    int rc = vsr_engine_create(m, opts, 0, 1, &e, err, sizeof err);
+    if (rc) {
+        stats->rc = rc;
+        if (opts->verbose) fprintf(stderr, "vsr_bfs: %s\n", err);
+        return rc;
+    }
+    const double t_setup = now_s() - t0;
+    std::vector<uint32_t> cands(4096);
+    int n = 0;
+    rc = vsr_bfs_sharded(e, opts, 0, stats, trace_out ? cands.data() : nullptr, &n, cands.size());
+    replay_counterexample(m, rc, cands.data(), n, stats, trace_out, trace_actions, trace_cap);
+    stats->rc = rc;
+    stats->seconds_setup = t_setup;
+    stats->seconds_total = now_s() - t0;
+    if (rc != VSR_RC_OK && rc != VSR_RC_VIOLATION && rc != VSR_RC_DEADLOCK && e->last_error[0] && opts->verbose) fprintf(stderr, "vsr_bfs: %s\n", e->last_error);
+    vsr_engine_destroy(e);
+    return rc;
+}
+
+int vsr_engine_build_trace(VsrEngine* e, uint64_t local_id, void* trace_out, uint8_t* trace_actions, size_t trace_cap) {
+    if (e->world != 1) return -VSR_RC_ERROR; /* multi-rank chains are walked by all ranks together (vsr_bfs_sharded) */
+    std::vector<uint32_t> cands;
+    if (walk_trace(e, local_id, cands)) return -VSR_RC_ERROR;
+    return vsr_replay_candidates(e->m, cands.data(), (int)cands.size(), trace_out, trace_actions, trace_cap);
 }
 
 } /* extern "C" */

@@ -169,7 +169,8 @@ class GpuEngine:
     def run(self, max_depth: int = 0, max_seconds: float = 0.0, max_states: int = 0, stop_on_violation: bool = True,
             want_trace: bool = True, part_states: int = 0, verbose: bool = False, checkpoint_path: Optional[str] = None,
             recover_path: Optional[str] = None, checkpoint_seconds: float = 0.0) -> ShardedResult:
-        """checkpoint_path / recover_path: every rank writes / reads ``<path>.rank<r>`` at level boundaries (TLC -checkpoint / -recover)"""
+        """checkpoint_path / recover_path: written / read at level boundaries (TLC -checkpoint / -recover); with several ranks
+        every rank uses ``<path>.rank<r>``"""
         o = self._opts
         o.max_depth, o.max_seconds, o.max_states = max_depth, max_seconds, max_states
         o.stop_on_violation, o.verbose = int(stop_on_violation), int(verbose)
