@@ -166,8 +166,8 @@ def check_audit(a, level, size):
 
 def engine_bfs(pkg, mc, max_depth=0, table=1 << 23, frontier=1 << 21, collect=True, audit=True, **kw):
     """The BFS pumped level by level through GpuEngine (reset / seed / expand / finish), every level audited.  Returns an
-    object with the fields assert_same_exploration compares, and per level (size, generated, fingerprint sum, fingerprint
-    xor, words sum, words xor)."""
+    object with the fields assert_same_exploration compares and the seen-set's fingerprint collisions per level, and per
+    level (size, generated, fingerprint sum, fingerprint xor, words sum, words xor)."""
     from vsr_tlaplus_b200 import dist as vdist
     keep = kw.pop("keep", False)  # leave the engine open (res.engine) for the caller
     eng = vdist.GpuEngine(mc, 0, 1, table_capacity=table, frontier_capacity=frontier, keep_trace=kw.pop("keep_trace", False),
@@ -176,7 +176,7 @@ def engine_bfs(pkg, mc, max_depth=0, table=1 << 23, frontier=1 << 21, collect=Tr
         eng.reset()
         eng.seed()
         li = eng.finish()
-        sizes, gens, rows, ties, generated, complete = [], [], [], 0, int(li.generated), False
+        sizes, gens, colls, rows, ties, generated, complete = [], [], [], [], 0, int(li.generated), False
         while True:
             assert li.error_code == 0 and li.overflow == 0, ("depth", len(sizes) + 1, "error", li.error_code, "overflow", li.overflow,
                                                              "new states", li.new_states)
@@ -185,6 +185,7 @@ def engine_bfs(pkg, mc, max_depth=0, table=1 << 23, frontier=1 << 21, collect=Tr
                 complete = True
                 break
             sizes.append(int(li.new_states))
+            colls.append(int(li.collisions))
             if audit:
                 a = eng.audit()
                 check_audit(a, len(sizes), sizes[-1])
@@ -196,7 +197,7 @@ def engine_bfs(pkg, mc, max_depth=0, table=1 << 23, frontier=1 << 21, collect=Tr
             gens.append(int(li.generated))
             generated += int(li.generated)
         res = types.SimpleNamespace(rc=0, error_code=0, level_sizes=sizes, level_generated=(gens + [0])[:len(sizes)] if not complete else gens,
-                                    distinct=sum(sizes), generated=generated, depth=len(sizes), h2_ties=ties, complete=complete,
+                                    distinct=sum(sizes), generated=generated, depth=len(sizes), h2_ties=ties, complete=complete, level_collisions=colls,
                                     queue=0 if complete else sizes[-1], levels=[eng.collected(d) for d in range(1, len(sizes) + 1)] if collect else [],
                                     engine=eng)
         if not keep:
@@ -210,11 +211,12 @@ def engine_bfs(pkg, mc, max_depth=0, table=1 << 23, frontier=1 << 21, collect=Tr
 _oracle = {}
 
 
-def oracle(R, V, L, depth):
-    if (R, V, L, depth) not in _oracle:
-        q = orc.params(R, V, L, symmetry=V > 1)
-        _oracle[(R, V, L, depth)] = (q, orc.bfs(q, workers=8, max_depth=depth, keep_trace=False, digests=True))
-    return _oracle[(R, V, L, depth)]
+def oracle(R, V, L, depth, symmetry=True):
+    key = (R, V, L, depth, symmetry and V > 1)
+    if key not in _oracle:
+        q = orc.params(R, V, L, symmetry=key[-1])
+        _oracle[key] = (q, orc.bfs(q, workers=8, max_depth=depth, keep_trace=False, digests=True))
+    return _oracle[key]
 
 
 def assert_parity(pkg, R, V, L, depth, res, mc):
@@ -276,8 +278,8 @@ def run_in_child(so, R, V, L, depth, out, collect=True, **kw):
     return types.SimpleNamespace(**d), rows, sets
 
 
-def assert_child_parity(R, V, L, depth, res, sets):
-    q, o = oracle(R, V, L, depth)
+def assert_child_parity(R, V, L, depth, res, sets, symmetry=True):
+    q, o = oracle(R, V, L, depth, symmetry)
     assert res.level_sizes == o.level_sizes
     assert res.level_generated[:len(o.level_generated)] == o.level_generated
     assert (res.distinct, res.generated, res.depth, res.h2_ties) == (o.distinct, o.generated, o.depth, o.h2_ties)

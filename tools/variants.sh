@@ -33,4 +33,5 @@ build bucket4 "-DVSR_BUCKET=4"           # 4-entry bucket, two 256-bit loads iss
 fi
 
 build qps1 "-DVSR_QPS=1"                 # correctness variant (pool overflow path): VSR_B200_LIB=...qps1.so python -m pytest tests/test_gpu_parity.py -k "3-2-2 or deterministic"
+build weakfp "-DVSR_WEAK_FP_BITS=16"     # correctness variant (16-bit fingerprints: collisions everywhere, kept apart by the check hash; tests/test_fp_collisions.py)
 rm -f $OUT/vsr_group.o

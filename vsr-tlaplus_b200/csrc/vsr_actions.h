@@ -673,6 +673,17 @@ template <class L> struct Ops {
  */
 constexpr uint64_t FP64_POLY = 0x911498AE0E66BAD6ULL;
 
+/* Test builds only (tests/test_fp_collisions.py, tools/variants.sh "weakfp"): -DVSR_WEAK_FP_BITS=k keeps the low k bits
+   of both fingerprint forms, host and device alike, so that different states share fingerprints all the time and the
+   seen-set has to keep them apart by their check hash.  k = 0 gives every state fingerprint 0 (1 after the usual remap):
+   one probe chain.  The product build never defines it. */
+#ifdef VSR_WEAK_FP_BITS
+static_assert(VSR_WEAK_FP_BITS >= 0 && VSR_WEAK_FP_BITS <= 63, "VSR_WEAK_FP_BITS: 0..63");
+VSR_HD uint64_t fp64_weaken(uint64_t fp) { return fp & ((1ull << VSR_WEAK_FP_BITS) - 1ull); }
+#else
+VSR_HD uint64_t fp64_weaken(uint64_t fp) { return fp; }
+#endif
+
 inline void fp64_build_table(uint64_t tab[256]) {
     uint64_t power[72];
     uint64_t t = 0x8000000000000000ULL;
@@ -701,7 +712,7 @@ template <class L> VSR_HD uint64_t fp64_view(const uint64_t* __restrict__ tab, c
             x >>= 8;
         }
     }
-    return fp;
+    return fp64_weaken(fp);
 }
 
 /* Slicing-by-8: the same function eight bytes per step.  S[j][b] = state after byte b followed by j zero bytes,
@@ -761,7 +772,7 @@ VSR_UNROLL
         const uint32_t y = x ^ (uint32_t)fp;
         fp = (fp >> 32) ^ s8[3 * 256 + (y & 0xFF)] ^ s8[2 * 256 + ((y >> 8) & 0xFF)] ^ s8[1 * 256 + ((y >> 16) & 0xFF)] ^ s8[(y >> 24) & 0xFF];
     }
-    return fp;
+    return fp64_weaken(fp);
 }
 template <class L, class W> VSR_HD uint64_t fp64_view8(const uint64_t* __restrict__ s8, const W& w, bool use_view) {
     return use_view ? fp64_view8_t<L, true>(s8, w) : fp64_view8_t<L, false>(s8, w);
