@@ -185,7 +185,9 @@ int vsr_engine_expand_part(VsrEngine* e, uint64_t first, uint64_t count);
  * this launch pushed to rank d (tell rank d: it is its drain_counts[this rank] of the next step).  Returns after the
  * kernel has completed, i.e. after the pushed records have landed. */
 int vsr_engine_step(VsrEngine* e, uint64_t first, uint64_t count, int parity, const uint32_t* drain_counts, uint32_t* sent_out);
-/* inserts records (device pointer, layout above) as states of the level being generated (Init; tests) */
+/* inserts n records (device pointer, 16-byte aligned, layout above; n <= UINT32_MAX) as states of the level being
+ * generated: one launch of the wavefront kernel with no frontier share that drains them, i.e. the insert every successor
+ * of the BFS goes through (vsr_engine_seed_init inserts Init the same way).  Tests inject records here. */
 int vsr_engine_insert_records(VsrEngine* e, const void* dev_records, uint64_t n);
 /* finishes the level: resolves ties, swaps frontiers; writes this rank's level numbers */
 typedef struct VsrLevelInfo {

@@ -23,7 +23,6 @@ build() { # name, flags
 }
 build base ""                            # the default: one block of up to 32 warps per SM, pool fast path
 build warps16 "-DVSR_FORCE_WARPS=16"     # two blocks of 16 warps per SM (the shape until the re-entry session's A/B: +13 % kernel time)
-build invskip "-DVSR_EXP_INVSKIP"        # inline invariant only after the action groups that can falsify it (they rewrite a log / acknowledge a value)
 build nopushfast "-DVSR_EXP_NO_PUSHFAST" # pool layout with the per-pair bound test always (+0.8 %)
 build roundclk "-DVSR_EXP_ROUNDCLK"      # per-level split of the expand warps' cycles (end-of-round barrier, scan barriers, batches, scan) on stderr
 build passes1 "-DVSR_ROUND_PASSES=1"     # one scan pass per round (the shape before profiles/round_tail_h100.md)

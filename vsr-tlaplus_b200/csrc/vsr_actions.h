@@ -526,12 +526,6 @@ template <class L> struct Ops {
         }
     }
 
-    /* Can action group g turn a state that satisfies every invariant below into one that violates one?  They read rep_log and
-       aux_client_acked (and the test hook rep_commit_number) only: SendSV (4), ReceiveSV (5), SendGetState (10) and
-       ReceiveNewState (12) replace or truncate a log, ExecuteOp (9) acknowledges a value and ReceivePrepare (7) / ExecuteOp move a
-       commit number; ReceiveClientRequest (6) and ReceivePrepare only append.  Every other group leaves those fields alone. */
-    static VSR_HD constexpr bool may_falsify(int g) { return g == 4 || g == 5 || g == 7 || g == 9 || g == 10 || g == 12; }
-
     /* invariants, VSR.tla:926-952; returns 0 if all selected hold, else the mask bit of the violated one */
     template <class W> static VSR_HD int invariant(const RunCfg& run, const W& w) {
         if (run.invariant & 256) { /* test hook, not a spec invariant (only reachable through vsr_model_create): "no replica has

@@ -60,7 +60,6 @@ struct VsrEngine {
     bool peer_is_ipc[vsr::MAX_WORLD] = {false};
     uint8_t* stage = nullptr;
     VsrGroup* group = nullptr;
-    int push_direct = 0;         /* VSR_B200_PUSH=direct */
     /* BFS position */
     int cur = 0;                 /* which frontier buffer is the current level */
     uint64_t n_cur = 0;          /* states in it */

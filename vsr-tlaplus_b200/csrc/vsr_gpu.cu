@@ -70,7 +70,44 @@ void fill_params(VsrEngine* e, ExpandParams& p) {
     p.world = e->world;
     p.owner_shift = e->owner_shift;
     p.push_cap = e->inbox_cap;
-    p.push_direct = e->push_direct;
+}
+
+/* One launch of the wavefront kernel over p.n_in frontier states and p.drain_total records to insert: clears the
+   per-launch counters, sizes the grid for the larger of the two, and brackets the launch with ev0 / ev1 (the caller
+   decides whether the level's kernel time counts it). */
+static int launch_expand(VsrEngine* e, const ExpandParams& p) {
+    CK(cudaMemsetAsync(&e->ctr->work_next, 0, sizeof(DevCounters) - offsetof(DevCounters, work_next), e->stream)); /* work_next, drain_next, send_count[] */
+    const uint64_t spb = (uint64_t)e->g->states_per_block;
+    const uint64_t want_blocks = (std::max<uint64_t>(p.n_in, p.drain_total) + spb - 1) / spb;
+    const uint64_t max_blocks = (uint64_t)e->sms * e->blocks_per_sm; /* persistent: whole multiples of the SM count */
+    int grid = (int)(want_blocks < max_blocks ? want_blocks : max_blocks);
+    if (grid < 1) grid = 1;
+    CK(cudaEventRecord(e->ev0, e->stream));
+    CK(e->g->launch_expand(p, grid, e->stream));
+    CK(cudaEventRecord(e->ev1, e->stream));
+    e->st.kernel_launches++;
+    return 0;
+}
+
+/* Inserts n records (device memory, 16-byte aligned; the layout of vsr_engine_record_bytes) as states of the level being
+   generated: a launch with no frontier share whose drain is the records.  The same insert, tie list, invariant and staging
+   code as every successor of the BFS (Expander::commit). */
+static int insert_records(VsrEngine* e, const void* recs, uint64_t n) {
+    if (n > UINT32_MAX) { /* drain_n[] counts 32 bits */
+        snprintf(e->last_error, sizeof e->last_error, "insert records: %llu records, at most %u per call", (unsigned long long)n, UINT32_MAX);
+        return VSR_RC_ERROR;
+    }
+    if ((uintptr_t)recs & 15) { /* the drain reads them with 16-byte loads */
+        snprintf(e->last_error, sizeof e->last_error, "insert records: %p is not 16-byte aligned", recs);
+        return VSR_RC_ERROR;
+    }
+    ExpandParams p;
+    fill_params(e, p);
+    p.n_in = 0;
+    p.drain[0] = (const uint8_t*)recs;
+    p.drain_n[0] = (unsigned)n;
+    p.drain_total = n;
+    return launch_expand(e, p);
 }
 
 extern "C" {
@@ -100,7 +137,6 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     while ((1 << lg) < world) lg++;
     e->owner_shift = world > 1 ? 64 - lg : 64;
     e->device = opts->device;
-    if (const char* pm = getenv("VSR_B200_PUSH")) e->push_direct = strcmp(pm, "direct") == 0;
     memset(&e->st, 0, sizeof e->st);
     auto bail = [&](const char* what, cudaError_t c) {
         std::string msg = std::string(what) + ": " + cudaGetErrorString(c);
@@ -205,14 +241,7 @@ int vsr_engine_seed_init(VsrEngine* e) {
     h->tm = make_trec(ROOT_GID, 0) | (1ull << 56); /* no parent; stands for one generated state */
     CK(cudaMemcpyAsync(e->init_rec, rec.data(), rec.size(), cudaMemcpyHostToDevice, e->stream));
     e->st.bytes_h2d += rec.size();
-    InsertParams q;
-    fill_params(e, q.e);
-    q.e.level = 1;
-    q.recs = e->init_rec;
-    q.n = 1;
-    CK(e->g->launch_insert(q, e->stream));
-    e->st.kernel_launches++;
-    return 0;
+    return insert_records(e, e->init_rec, 1); /* untimed: the level's kernel time starts with the first expansion */
 }
 
 /* One launch of the wavefront kernel: expand frontier states [first, first + count) of the current level (count = 0:
@@ -258,18 +287,8 @@ int vsr_engine_step(VsrEngine* e, uint64_t first, uint64_t count, int parity, co
     }
     if (sent_out) memset(sent_out, 0, sizeof(uint32_t) * e->world);
     if (count == 0 && drain_total == 0) return 0;
-    CK(cudaMemsetAsync(&e->ctr->work_next, 0, sizeof(DevCounters) - offsetof(DevCounters, work_next), e->stream)); /* work_next, drain_next, send_count[] */
-    const uint64_t spb = (uint64_t)e->g->states_per_block;
-    uint64_t want_blocks = (count + spb - 1) / spb;
-    const uint64_t drain_blocks = (drain_total + spb - 1) / spb;
-    if (drain_blocks > want_blocks) want_blocks = drain_blocks;
-    const uint64_t max_blocks = (uint64_t)e->sms * e->blocks_per_sm; /* persistent: whole multiples of the SM count */
-    int grid = (int)(want_blocks < max_blocks ? want_blocks : max_blocks);
-    if (grid < 1) grid = 1;
-    CK(cudaEventRecord(e->ev0, e->stream));
-    CK(e->g->launch_expand(p, grid, e->stream));
-    CK(cudaEventRecord(e->ev1, e->stream));
-    e->st.kernel_launches++;
+    const int rc = launch_expand(e, p);
+    if (rc) return rc;
     if (e->world > 1 && sent_out) {
         CK(cudaMemcpyAsync(sent_out, e->ctr->send_count, sizeof(uint32_t) * e->world, cudaMemcpyDeviceToHost, e->stream));
         e->st.bytes_d2h += sizeof(uint32_t) * e->world;
@@ -295,14 +314,8 @@ int vsr_engine_insert_records(VsrEngine* e, const void* dev_records, uint64_t n)
         if (rc) return rc;
     }
     if (n == 0) return 0;
-    InsertParams q;
-    fill_params(e, q.e);
-    q.recs = (const uint8_t*)dev_records;
-    q.n = n;
-    CK(cudaEventRecord(e->ev0, e->stream));
-    CK(e->g->launch_insert(q, e->stream));
-    CK(cudaEventRecord(e->ev1, e->stream));
-    e->st.kernel_launches++;
+    const int rc = insert_records(e, dev_records, n);
+    if (rc) return rc;
     CK(cudaEventSynchronize(e->ev1));
     float ms = 0;
     cudaEventElapsedTime(&ms, e->ev0, e->ev1);

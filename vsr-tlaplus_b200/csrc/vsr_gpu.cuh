@@ -106,18 +106,12 @@ struct ExpandParams {
        buffer when the host moves them with a collective.  Slots are taken from the local counters ctr->send_count[d]. */
     uint8_t* push[MAX_WORLD];
     unsigned long long push_cap; /* records per segment */
-    int push_direct;             /* 1: every lane stores its own record with 16-byte stores (VSR_B200_PUSH=direct); 0: staged + TMA bulk store */
     /* records received from rank s in the previous step (the other half of the double-buffered inbox): inserted by this
-       launch after its share of the frontier */
+       launch after its share of the frontier.  Init and vsr_engine_insert_records come this way too, as drain[0] of a
+       launch with no frontier share */
     const uint8_t* drain[MAX_WORLD];
     unsigned int drain_n[MAX_WORLD];
     unsigned long long drain_total;
-};
-
-struct InsertParams {
-    const uint8_t* recs;
-    unsigned long long n;
-    ExpandParams e;              /* table / out / trace / counters as above */
 };
 
 /* ------------------------------------------------------------------ primitives */
@@ -342,8 +336,9 @@ template <class L> struct ExpandCfg {
  * (2) guards in a run-time loop over candidates with one ballot + barrier per group: 75 warp instructions per
  * (32 states, candidate) for slot decoding and shared-memory field reads; (3) this form: 16 per candidate.
  */
-/* MULTI: the instantiation for several GPUs (push_records in emit, drain after the rounds).  The one-GPU instantiation has none
-   of that code: it costs the hot path registers (380 vs 140 bytes of spills in emit at the 64-register budget). */
+/* MULTI: the instantiation for several GPUs (push_records in emit, drain after the rounds), and for every launch that inserts
+   records (Init, vsr_engine_insert_records).  The one-GPU expansion has none of that code: it costs the hot path registers
+   (380 vs 140 bytes of spills in emit at the 64-register budget). */
 template <class L, bool MULTI> struct Expander {
     typedef Ops<L> O_;
     typedef typename ExpandCfg<L>::Smem Smem;
@@ -462,15 +457,6 @@ template <class L, bool MULTI> struct Expander {
         base = __shfl_sync(0xffffffffu, base, mymask ? __ffs(mymask) - 1 : 0);
         const bool fits = send_to >= 0 && (unsigned long long)base + (unsigned)cnt <= P.push_cap;
         if (send_to >= 0 && !fits && rnk == 0) atomicExch(&P.ctr->overflow, 3);
-        if (P.push_direct) { /* fallback / A-B: no staging, four half-sector stores per lane */
-            if (fits) {
-                uint4* d = reinterpret_cast<uint4*>(P.push[send_to] + (size_t)(base + (unsigned)rnk) * RB);
-                VSR_UNROLL
-                for (int q = 0; q < L::NW / 4; q++) d[q] = make_uint4(v.w[4 * q], v.w[4 * q + 1], v.w[4 * q + 2], v.w[4 * q + 3]);
-                d[L::NW / 4] = make_uint4((uint32_t)fp, (uint32_t)(fp >> 32), (uint32_t)tm, (uint32_t)(tm >> 32));
-            }
-            return;
-        }
         const int pos = off + rnk, total = __popc(senders);
         uint32_t* sbuf = &S.stage[(SROWS - 32) * L::NW];
         for (int lo = 0; lo < total; lo += CAPREC) {
@@ -493,12 +479,13 @@ template <class L, bool MULTI> struct Expander {
     }
 
     /* the seen-set insert of one state per lane and everything after it — tie list, inline invariant, compaction of the
-       survivors into the warp's staging area, flush — shared by the expansion (emit) and by the records received from
-       peers (drain).  Returns this lane's counts for the run's statistics: successors generated (low half) | seen-set
-       probes (high half); the caller keeps the running sums in registers (a warp reduction per batch cost 25 shuffles) */
+       survivors into the warp's staging area, flush — shared by the expansion (emit) and by the records of the drain
+       (received from peers, Init, injected records): the only insert of a state in the library.  Returns this lane's
+       counts for the run's statistics: successors generated (low half) | seen-set probes (high half); the caller keeps
+       the running sums in registers (a warp reduction per batch cost 25 shuffles) */
     static __device__ __forceinline__ unsigned long long commit(const ExpandParams& P, Stage& S, int lane, const RegRow<L::NW>& v, bool live, uint64_t fp,
                                                                 uint32_t chk, uint32_t auxkey, unsigned long long home, const Probe& first, unsigned long long trec,
-                                                                unsigned mult, bool check_inv = true) {
+                                                                unsigned mult) {
         unsigned gen = 0, probes = 0, coll = 0;
         int sn = SROWS == 32 ? 0 : S.sn;
         bool isnew = false;
@@ -509,7 +496,7 @@ template <class L, bool MULTI> struct Expander {
             const int r = table_insert_from(P.table, P.table_cap, home, first, fp, meta, probes, coll);
             isnew = r == INS_NEW;
             if (r == INS_FULL) atomicExch(&P.ctr->overflow, 4);
-            if (isnew && check_inv) bad = O_::invariant(P.run, v);
+            if (isnew) bad = O_::invariant(P.run, v);
             if (coll) atomicAdd(&P.ctr->collisions, (unsigned long long)coll); /* never seen so far */
             if (r == INS_TIE) {
                 atomicAdd(&P.ctr->ties, 1ull);
@@ -555,7 +542,7 @@ template <class L, bool MULTI> struct Expander {
 
     /* fingerprint and route one successor per lane: the part of apply that does not depend on the action */
     static __device__ __noinline__ unsigned long long emit(const ExpandParams& P, Smem& B, Stage& S, int lane, const Row n, int mult,
-                                                           int cand, int si, bool act, bool check_inv) {
+                                                           int cand, int si, bool act) {
         int send_to = -1;
         uint64_t fp = 0;
         uint32_t chk = 0, auxkey = 0;
@@ -593,10 +580,11 @@ template <class L, bool MULTI> struct Expander {
             __syncwarp(); /* every lane has read its scratch row: that half of the staging area may now carry outgoing records */
             push_records(P, S, lane, v, send_to, fp, trec | ((uint64_t)(unsigned)mult << 56));
         }
-        return commit(P, S, lane, v, live, fp, chk, auxkey, home, first, trec, (unsigned)mult, check_inv);
+        return commit(P, S, lane, v, live, fp, chk, auxkey, home, first, trec, (unsigned)mult);
     }
 
-    /* ---- drain: one record received from a peer per lane (world > 1), after this block's share of the frontier.  The
+    /* ---- drain: one record per lane, after this block's share of the frontier: received from a peer (world > 1), or
+       Init and the records of vsr_engine_insert_records (a launch with no frontier share, at any world size).  The
        sender computed the fingerprint; check hash and aux key are recomputed from the words; then the same seen-set insert
        / invariant / staging as a local successor.  drain_begin issues the header and bucket loads, drain_end consumes them.
        One record in flight per lane: more (2 or 4), or pipelining a chunk under every batch of the expansion, costs
@@ -787,13 +775,7 @@ template <class L, bool MULTI> struct Expander {
         const Row n = scratch(S, lane);
         int mult = 0;
         if (act) mult = O_::template step_grp<true, G>(P.run, parent, cand, n);
-#ifdef VSR_EXP_INVSKIP
-        /* the invariants read the replicas' logs and the acknowledgements only (VSR.tla:933-950): a successor of a state that
-           satisfies them can violate them only through an action that rewrites a log or acknowledges a value (Ops::may_falsify) */
-        return emit(P, B, S, lane, n, mult, cand, si, act, O_::may_falsify(G));
-#else
-        return emit(P, B, S, lane, n, mult, cand, si, act, true);
-#endif
+        return emit(P, B, S, lane, n, mult, cand, si, act);
     }
     /* one batch of <= 32 queued pairs of group G, pool[b .. b + k) (all of one pass) */
     template <int G> static __device__ __forceinline__ unsigned long long batch(const ExpandParams& P, Smem& B, Stage& S, int lane, int b,
@@ -942,78 +924,6 @@ template <class L, bool MULTI> __global__ void __launch_bounds__(ExpandCfg<L>::W
     X.finish();
 }
 
-/* ------------------------------------------------------------------ insert kernel (records from peers, and Init) */
-
-template <class L> __global__ void __launch_bounds__(256) insert_kernel(const InsertParams Q) {
-    const ExpandParams& P = Q.e;
-    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int lane = threadIdx.x & 31;
-    const bool have = i < Q.n;
-    bool isnew = false;
-    const uint8_t* rec = Q.recs + (have ? i : 0) * (L::BYTES + sizeof(RecHdr));
-    const uint32_t* n = (const uint32_t*)rec;
-    const RecHdr* h = (const RecHdr*)(rec + L::BYTES);
-    unsigned probes = 0, coll = 0, nties = 0;
-    unsigned long long gen = 0;
-    uint64_t parent = 0;
-    uint32_t cand = 0;
-    if (have) {
-        /* check hash and aux key are computed here from the words; the header carries the fingerprint, the trace record and mult */
-        const uint64_t meta = make_meta(P.level, Ops<L>::aux_key(n), check_hash<L>(n, P.run.use_view != 0));
-        const int r = table_insert(P.table, P.table_cap, h->fp, meta, probes, coll);
-        isnew = r == INS_NEW;
-        if (r == INS_FULL) atomicExch(&P.ctr->overflow, 4);
-        gen = (h->tm >> 56) & 0xFu;
-        parent = (h->tm >> 12) & ((1ull << 44) - 1ull);
-        cand = (uint32_t)(h->tm & 0xFFFu);
-        if (r == INS_TIE) {
-            nties = 1;
-            const unsigned long long t = atomicAdd(&P.ctr->tie_count, 1ull);
-            if (t < P.tie_cap) {
-                TieRec tr;
-                tr.fp = h->fp; tr.parent = parent; tr.auxkey = (uint32_t)((meta >> 32) & 0xFFFFFF); tr.cand = cand;
-                tr.check = (uint32_t)meta; tr._pad = 0;
-                uint8_t* dst = P.ties + t * (sizeof(TieRec) + L::BYTES);
-                *(TieRec*)dst = tr;
-                for (int j = 0; j < L::NW; j++) ((uint32_t*)(dst + sizeof(TieRec)))[j] = n[j];
-            } else atomicExch(&P.ctr->overflow, 2);
-        }
-    }
-    /* per-warp totals: one atomic per counter per warp, not per record */
-    for (int o = 16; o; o >>= 1) {
-        gen += __shfl_xor_sync(0xffffffffu, gen, o);
-        probes += __shfl_xor_sync(0xffffffffu, probes, o);
-        coll += __shfl_xor_sync(0xffffffffu, coll, o);
-        nties += __shfl_xor_sync(0xffffffffu, nties, o);
-    }
-    if (lane == 0) {
-        if (gen) atomicAdd(&P.ctr->generated, gen);
-        if (probes) atomicAdd(&P.ctr->probes, (unsigned long long)probes);
-        if (coll) atomicAdd(&P.ctr->collisions, (unsigned long long)coll);
-        if (nties) atomicAdd(&P.ctr->ties, (unsigned long long)nties);
-    }
-    const unsigned newmask = __ballot_sync(0xffffffffu, isnew);
-    if (newmask) {
-        unsigned long long base = 0;
-        const int leader = __ffs(newmask) - 1;
-        if (lane == leader) base = atomicAdd(&P.ctr->out_count, (unsigned long long)__popc(newmask));
-        base = __shfl_sync(0xffffffffu, base, leader);
-        if (isnew) {
-            const unsigned long long pos = base + __popc(newmask & ((1u << lane) - 1u));
-            if (pos < P.out_cap) {
-                uint32_t* dst = out_state<L::NW>(P, pos);
-                for (int j = 0; j < L::NW; j++) dst[j] = n[j];
-                if (P.trace && P.out_base + pos < P.trace_cap) P.trace[P.out_base + pos] = make_trec(parent, cand);
-                const int bad = Ops<L>::invariant(P.run, n);
-                if (bad) {
-                    atomicMin(&P.ctr->viol_id, P.out_base + pos);
-                    atomicOr(&P.ctr->viol_which, bad);
-                }
-            } else atomicExch(&P.ctr->overflow, 1);
-        }
-    }
-}
-
 /* VIEW-tie patch pass (SURVEY H2; only launched for a level that reported ties).  `ties` holds, sorted by fp, ONE
    record per tied fingerprint: the smallest (aux_key, parent, candidate) among the late arrivals.  Every state of the
    new level looks itself up; if a tie record beats the first arrival's aux_key, the state and its trace record are
@@ -1051,21 +961,26 @@ template <class L> __global__ void patch_ties_kernel(const ExpandParams P, const
     }
 }
 
-/* membership query (tests / golden-trace cross-check): meta of the entry holding (fp, check), 0 if absent */
-static __global__ void lookup_kernel(const uint64_t* table, unsigned long long cap, uint64_t fp, uint32_t check, unsigned long long* meta_out) {
+/* meta of the seen-set entry holding (fp, check), 0 if absent (an entry's meta carries its level, >= 1).  The insert's
+   probe order: entry by entry from the home bucket; the first empty slot ends the chain */
+__device__ __forceinline__ uint64_t table_lookup(const uint64_t* table, unsigned long long cap, uint64_t fp, uint32_t check) {
     unsigned long long h = table_home(cap, fp);
     for (unsigned long long i = 0; i < cap; i++) {
         const uint64_t e0 = table[2 * h], e1 = table[2 * h + 1];
-        if (e0 == 0) { *meta_out = 0; return; }
-        if (e0 == fp && (uint32_t)e1 == check) { *meta_out = e1; return; }
+        if (e0 == 0) return 0;
+        if (e0 == fp && (uint32_t)e1 == check) return e1;
         if (++h >= cap) h = 0;
     }
-    *meta_out = 0;
+    return 0;
+}
+
+/* membership query (tests / golden-trace cross-check) */
+static __global__ void lookup_kernel(const uint64_t* table, unsigned long long cap, uint64_t fp, uint32_t check, unsigned long long* meta_out) {
+    *meta_out = table_lookup(table, cap, fp, check);
 }
 
 /* per-level audit (tests, vsr_engine_audit_level): seen-set entries tagged with a level, and the level's frontier looked up
-   in the seen-set with the insert's probe order (entry by entry from the home bucket; the first empty slot ends the chain),
-   plus order-independent digests of the frontier and of the tagged entries' fingerprints */
+   in the seen-set (table_lookup), plus order-independent digests of the frontier and of the tagged entries' fingerprints */
 struct AuditSums {
     unsigned long long tagged, found, fp_sum, fp_xor, words_sum, words_xor, tagged_fp_sum, tagged_fp_xor;
 };
@@ -1103,16 +1018,7 @@ template <class L> __global__ void audit_frontier_kernel(const ExpandParams P, u
         uint64_t fp = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
         if (fp == 0) fp = 1;
         const uint32_t chk = check_hash<L>(w, P.run.use_view != 0);
-        unsigned long long h = table_home(P.table_cap, fp);
-        for (unsigned long long k = 0; k < P.table_cap; k++) {
-            const uint64_t e0 = P.table[2 * h], e1 = P.table[2 * h + 1];
-            if (e0 == 0) break;
-            if (e0 == fp && (uint32_t)e1 == chk) {
-                found += (int)(e1 >> 56) == P.level;
-                break;
-            }
-            if (++h >= P.table_cap) h = 0;
-        }
+        found += (int)(table_lookup(P.table, P.table_cap, fp, chk) >> 56) == P.level;
         fs += mix64(fp);
         fx ^= mix64(fp);
         ws += hw;

@@ -16,7 +16,6 @@ struct GpuOps {
     size_t expand_smem;
     int states_per_block;
     cudaError_t (*launch_expand)(const ExpandParams&, int grid, cudaStream_t);
-    cudaError_t (*launch_insert)(const InsertParams&, cudaStream_t);
     cudaError_t (*launch_patch)(const ExpandParams&, const uint8_t* ties, unsigned long long ntie, unsigned long long n_out, cudaStream_t);
     int tie_bytes;
     cudaError_t (*prepare)(int* blocks_per_sm);
@@ -29,7 +28,7 @@ struct GpuOps {
 /* what a layout plug-in must have been compiled against: the version constant AND the shapes of the structs the kernels and the
    host exchange (a plug-in built from another revision of these headers must be rebuilt, never loaded) */
 inline int gpu_abi_value() {
-    return VSR_PLUGIN_ABI * 100000 + (int)((sizeof(ExpandParams) * 131 + sizeof(DevCounters) * 17 + sizeof(InsertParams) * 7 + sizeof(RecHdr) + VSR_BUCKET * 3) % 100000);
+    return VSR_PLUGIN_ABI * 100000 + (int)((sizeof(ExpandParams) * 131 + sizeof(DevCounters) * 17 + sizeof(RecHdr) + VSR_BUCKET * 3) % 100000);
 }
 
 template <class L> struct GpuThunks {
@@ -44,14 +43,9 @@ template <class L> struct GpuThunks {
         return e;
     }
     static cudaError_t launch_expand(const ExpandParams& p, int grid, cudaStream_t st) {
-        if (p.world > 1) expand_kernel<L, true><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
+        /* the one-GPU instantiation has no drain: records to insert (drain_total) need the MULTI one at any world size */
+        if (p.world > 1 || p.drain_total) expand_kernel<L, true><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
         else expand_kernel<L, false><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
-        return cudaGetLastError();
-    }
-    static cudaError_t launch_insert(const InsertParams& q, cudaStream_t st) {
-        if (q.n == 0) return cudaSuccess;
-        const unsigned blocks = (unsigned)((q.n + 255) / 256);
-        insert_kernel<L><<<blocks, 256, 0, st>>>(q);
         return cudaGetLastError();
     }
     static cudaError_t launch_patch(const ExpandParams& p, const uint8_t* ties, unsigned long long ntie, unsigned long long n_out, cudaStream_t st) {
@@ -72,7 +66,7 @@ template <class L> struct GpuThunks {
     static const GpuOps* get() {
         typedef ExpandCfg<L> Cfg;
         static const GpuOps ops = {chk, L::R, L::V, L::K, L::NW, L::BYTES, (int)(L::BYTES + sizeof(RecHdr)), sizeof(typename Cfg::Smem), Cfg::WARPS * 32,
-                                   launch_expand, launch_insert, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate,
+                                   launch_expand, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate,
                                    Cfg::WARPS, Cfg::BLOCKS, Cfg::PASSES, Expander<L, false>::SROWS, launch_audit};
         return &ops;
     }
