@@ -8,7 +8,7 @@
  * so the drop-in boundary is TLC's file + CLI surface (SURVEY §8b).  Each entry point below cites
  * the part of the reference it stands in for.  Plain pointers and sizes; caller owns every buffer;
  * no torch / C++ types.  Return codes follow TLC's exit statuses where one exists:
- *     0 ok, 11 deadlock, 12 safety (invariant) violation, 150 spec error, 151 config error,
+ *     0 ok, 11 deadlock, 12 safety (invariant) violation, 13 temporal property violated, 150 spec error, 151 config error,
  *     152 state space too large for the configured capacity, 153 system (CUDA) error, 255 other.
  */
 #ifndef VSR_B200_H
@@ -26,6 +26,7 @@ extern "C" {
 #define VSR_RC_OK 0
 #define VSR_RC_DEADLOCK 11
 #define VSR_RC_VIOLATION 12
+#define VSR_RC_LIVENESS 13
 #define VSR_RC_SPEC_ERROR 150
 #define VSR_RC_CONFIG_ERROR 151
 #define VSR_RC_TOO_LARGE 152
@@ -49,7 +50,8 @@ typedef struct VsrModelInfo {
     uint64_t spec_hash;                                 /* FNV-1a 64 of the .tla bytes (0 if none) */
     char value_names[VSR_MAX_V][32];                    /* model values of Values, cfg order */
     int32_t check_deadlock;                             /* CHECK_DEADLOCK in the cfg: 1 TRUE, 0 FALSE, -1 absent (TLC's default: check) */
-    int32_t _pad;
+    int32_t property;                                   /* bitmask of PROPERTY names: 1 ViewChangeCompletes (VSR.tla:964-965; needs
+                                                           SPECIFICATION Spec, whose WF_vars(Next) makes it meaningful) */
 } VsrModelInfo;
 
 /* ---- loading: TLC's `-config VSR.cfg VSR.tla` (SURVEY §8b; grammar of vsr-revisited/paper/VSR.cfg:1-39).
@@ -62,7 +64,11 @@ typedef struct VsrModelInfo {
 int vsr_load(const char* cfg_path, const char* tla_path, VsrModel** out, char* err, size_t errcap);
 /* same, from the text of a cfg file */
 int vsr_load_cfg_text(const char* cfg_text, const char* tla_path, VsrModel** out, char* err, size_t errcap);
-/* same, straight from constants (CONSTANTS of VSR.tla:92-96) */
+/* same, straight from constants (CONSTANTS of VSR.tla:92-96).  `invariant` is the INVARIANT bitmask of VsrModelInfo, plus
+ * bits only this entry point knows: 512 = check PROPERTY ViewChangeCompletes (as a cfg with SPECIFICATION Spec does); test
+ * hooks of the liveness pass, which leave the BFS as it is: 1024 = the pass checks []<>Q with Q = "some replica's
+ * rep_commit_number >= 1" instead (reachable not-Q states without successors exist), 2048 = in the pass every state
+ * without successors gets one extra successor, Init (with 1024: cycles through Init) */
 int vsr_model_create(int replica_count, int client_count, int value_count, int start_view_on_timer_limit,
                      int restart_empty_limit, int symmetry, int view, int invariant, VsrModel** out, char* err,
                      size_t errcap);
@@ -89,6 +95,9 @@ uint32_t vsr_aux_key(const VsrModel* m, const void* state);
  * fingerprint x an odd constant (FP64 is GF(2)-linear: its own high bits would route a rank's successors to a few peers only) */
 int vsr_owner_rank(uint64_t fingerprint, int world);
 int vsr_invariant(const VsrModel* m, const void* state);                 /* 0 = all hold, else mask bit of the violated one; VSR.tla:926-952 */
+/* 1 if the state predicate the liveness pass checks holds in `state`: AllReplicasMoveToSameView (VSR.tla:958-962), or the
+ * test hook's Q (vsr_model_create bit 1024); 0 if not */
+int vsr_property(const VsrModel* m, const void* state);
 int vsr_unpack(const VsrModel* m, const void* state, VsrFlatState* out);
 int vsr_pack(const VsrModel* m, const VsrFlatState* in, void* state_out);
 /* TLC value text of one state, format of state_transfer_violation_trace.txt (variables
@@ -154,12 +163,14 @@ typedef struct VsrStats {
     uint64_t records_sent, records_received; /* several GPUs: records this rank pushed to / drained from peers */
     double seconds_insert;                /* several GPUs: part of seconds_kernels spent in drain-only launches */
     int32_t levels_expanded;              /* frontiers expanded = valid entries of level_generated / level_ms */
-    int32_t _pad;
+    int32_t trace_loop;                   /* rc 13: the lasso's "Back to state K" (1-based; 0 = it ends in stuttering) */
 } VsrStats;
 
 typedef struct VsrEngine VsrEngine;
 
-/* One-call BFS on one GPU: engine creation (stats.seconds_setup), vsr_bfs_sharded on that world-1 engine, teardown.
+/* One-call BFS on one GPU: engine creation (stats.seconds_setup), vsr_bfs_sharded on that world-1 engine, then, when the
+ * model has a property and the BFS completed, vsr_engine_liveness (rc 13: the trace is the lasso, stats.trace_loop its
+ * back edge), teardown.
  * Fails loudly (153) when no CUDA device is usable — there is no CPU fallback.  If trace_out != NULL and a
  * violation/deadlock is found, writes the counterexample (packed states, trace_cap capacity) with its action ids;
  * stats.trace_len is its length, stats.violation_mask the invariants its last state violates. */
@@ -239,6 +250,37 @@ int vsr_expand_shape(const VsrModel* m, int* warps, int* blocks, int* passes, in
 /* Rebuild the behaviour from Init to local state id (world-1 engines; tests): the parent-chain walk of vsr_bfs_sharded,
  * replayed with vsr_replay_candidates.  Returns the number of states, or a negative status. */
 int vsr_engine_build_trace(VsrEngine* e, uint64_t local_id, void* trace_out, uint8_t* trace_actions, size_t trace_cap);
+
+/* ---- liveness: PROPERTY ViewChangeCompletes == []<>P under Spec's WF_vars(Next), P = AllReplicasMoveToSameView (DESIGN
+ * "Liveness").  When the model has the property, every finished level appends its not-P states to a store (words in HBM,
+ * continued in pinned host memory) and to a live index {fingerprint, check} -> store index.  After a COMPLETE BFS,
+ * vsr_engine_liveness sweeps the store deepest level first, keeping a state alive while some not-P successor other than
+ * itself is alive, until a sweep removes nothing.  The property is violated iff a not-P state has no successor but itself
+ * (stuttering forever is fair there) or some state stays alive (a not-P cycle).  One GPU (world 1) only. */
+#define VSR_MAX_SWEEPS 64
+typedef struct VsrLiveStats {
+    uint64_t stored;               /* not-P states in the store (all levels) */
+    uint64_t capacity;             /* states the store holds */
+    uint64_t bytes_hbm, bytes_host; /* store, live index and alive bits in HBM; the store's continuation in host memory */
+    uint64_t sinks;                /* not-P states without a successor other than themselves (first sweep) */
+    uint64_t survivors;            /* states alive after the last sweep */
+    uint64_t violation_index;      /* store index of the reported state (the smallest sink, else the smallest survivor) */
+    int32_t sweeps;                /* full passes over the store, the last of which removed nothing (or found sinks) */
+    int32_t rc;                    /* 0 holds, 13 violated, else an error status */
+    int32_t violation_level;       /* BFS depth of the reported state */
+    int32_t trace_loop;            /* "Back to state K" of the lasso (1-based); 0 = the lasso ends in stuttering */
+    int32_t trace_loop_action;     /* VSR_ACT_* of the step back to state K (0 = the test hook's edge to Init) */
+    int32_t trace_len;             /* candidates written to cands_out (the lasso has trace_len + 1 states; 0 = none kept) */
+    int32_t error_code;            /* E_* raised by a sweep (0 = none) */
+    int32_t _pad;
+    double seconds_total;          /* the whole liveness phase (sweeps and the lasso walk) */
+    double ms_sweep[VSR_MAX_SWEEPS]; /* device time of each sweep (CUDA events) */
+} VsrLiveStats;
+/* After vsr_bfs_sharded returned 0 with stats.complete on a world-1 engine of a model with a property: the sweeps and, on a
+ * violation, the lasso as a candidate chain from Init (cands_out[0 .. trace_len), replay with vsr_replay_candidates) whose
+ * last state steps back to state trace_loop (or stutters).  Returns 0 (holds), 13 (violated), 255 (the store disagrees with
+ * the BFS: stats.error_code), 151 (no property / not a complete one-GPU run) or 153. */
+int vsr_engine_liveness(VsrEngine* e, VsrLiveStats* stats, uint32_t* cands_out, size_t cands_cap);
 
 /* ---- several GPUs of one node (SURVEY §8e: TLC's `-workers` / distributed mode).  One rank per GPU — processes
  * (torchrun) or threads of one process — fingerprint space split by its high bits.  The ranks coordinate through a

@@ -86,7 +86,7 @@ class VsrModelInfo(C.Structure):
         ("symmetry", C.c_int32), ("view", C.c_int32), ("invariant", C.c_int32),
         ("state_bytes", C.c_int32), ("state_bits", C.c_int32), ("num_candidates", C.c_int32),
         ("spec_verified", C.c_int32), ("spec_hash", C.c_uint64), ("value_names", (C.c_char * 32) * VSR_MAX_V),
-        ("check_deadlock", C.c_int32), ("_pad", C.c_int32),
+        ("check_deadlock", C.c_int32), ("property", C.c_int32),
     ]
 
 
@@ -114,7 +114,20 @@ class VsrStats(C.Structure):
         ("bytes_table", C.c_uint64), ("bytes_frontier", C.c_uint64),
         ("bytes_h2d", C.c_uint64), ("bytes_d2h", C.c_uint64), ("seconds_setup", C.c_double),
         ("records_sent", C.c_uint64), ("records_received", C.c_uint64), ("seconds_insert", C.c_double),
-        ("levels_expanded", C.c_int32), ("_pad", C.c_int32),
+        ("levels_expanded", C.c_int32), ("trace_loop", C.c_int32),
+    ]
+
+
+VSR_MAX_SWEEPS = 64
+
+
+class VsrLiveStats(C.Structure):
+    _fields_ = [
+        ("stored", C.c_uint64), ("capacity", C.c_uint64), ("bytes_hbm", C.c_uint64), ("bytes_host", C.c_uint64),
+        ("sinks", C.c_uint64), ("survivors", C.c_uint64), ("violation_index", C.c_uint64),
+        ("sweeps", C.c_int32), ("rc", C.c_int32), ("violation_level", C.c_int32), ("trace_loop", C.c_int32),
+        ("trace_loop_action", C.c_int32), ("trace_len", C.c_int32), ("error_code", C.c_int32), ("_pad", C.c_int32),
+        ("seconds_total", C.c_double), ("ms_sweep", C.c_double * VSR_MAX_SWEEPS),
     ]
 
 
@@ -149,7 +162,7 @@ class VsrLevelAudit(C.Structure):
 # every symbol include/vsr_b200.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = [
     "vsr_load", "vsr_load_cfg_text", "vsr_model_create", "vsr_model_free", "vsr_model_info", "vsr_init", "vsr_successors", "vsr_enabled_candidates",
-    "vsr_canon", "vsr_fingerprint", "vsr_fingerprint_bytewise", "vsr_aux_key", "vsr_owner_rank", "vsr_invariant", "vsr_unpack", "vsr_pack", "vsr_state_to_tla",
+    "vsr_canon", "vsr_fingerprint", "vsr_fingerprint_bytewise", "vsr_aux_key", "vsr_owner_rank", "vsr_invariant", "vsr_property", "vsr_unpack", "vsr_pack", "vsr_state_to_tla",
     "vsr_flat_to_tla", "vsr_action_name", "vsr_action_location", "vsr_bfs", "vsr_engine_create", "vsr_engine_destroy",
     "vsr_engine_record_bytes", "vsr_engine_seed_init", "vsr_engine_expand", "vsr_engine_expand_part", "vsr_engine_step",
     "vsr_engine_insert_records", "vsr_engine_finish_level", "vsr_engine_frontier_size", "vsr_engine_read_frontier",
@@ -158,7 +171,7 @@ EXPORTED_SYMBOLS = [
     "vsr_group_open", "vsr_group_open_local", "vsr_group_close", "vsr_group_barrier", "vsr_group_allgather", "vsr_group_abort",
     "vsr_group_set_timeout", "vsr_group_rank", "vsr_group_world", "vsr_group_last_error",
     "vsr_engine_attach_group", "vsr_engine_attach_staged", "vsr_engine_detach", "vsr_engine_default_inbox_records",
-    "vsr_bfs_sharded", "vsr_bfs_multi",
+    "vsr_bfs_sharded", "vsr_bfs_multi", "vsr_engine_liveness",
 ]
 
 _lib = None
@@ -192,6 +205,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.vsr_owner_rank.argtypes = [u64, C.c_int]
     lib.vsr_aux_key.restype = C.c_uint32
     lib.vsr_invariant.argtypes = [vp, vp]
+    lib.vsr_property.argtypes = [vp, vp]
+    lib.vsr_engine_liveness.argtypes = [vp, C.POINTER(VsrLiveStats), C.POINTER(C.c_uint32), C.c_size_t]
     lib.vsr_unpack.argtypes = [vp, vp, C.POINTER(VsrFlatState)]
     lib.vsr_pack.argtypes = [vp, C.POINTER(VsrFlatState), vp]
     lib.vsr_state_to_tla.argtypes = [vp, vp, cp, C.c_size_t]
@@ -308,10 +323,18 @@ class CheckResult:
     seconds_insert: float = 0.0
     trace: List[Tuple[str, bytes]] = field(default_factory=list)  # (action name, packed state)
     levels: List[bytes] = field(default_factory=list)             # collect_levels: raw states per depth
+    # PROPERTY ViewChangeCompletes: the VsrLiveStats fields of the liveness pass ({} when it did not run), and for rc 13 the
+    # lasso's "Back to state K" (1-based into `trace`; 0 = the lasso ends in stuttering)
+    liveness: dict = field(default_factory=dict)
+    trace_loop: int = 0
 
     @property
     def violated(self) -> bool:
         return self.rc == 12
+
+    @property
+    def liveness_violated(self) -> bool:
+        return self.rc == 13
 
 
 class ModelChecker:
@@ -348,13 +371,18 @@ class ModelChecker:
     @classmethod
     def from_constants(cls, replica_count: int, value_count: int, start_view_on_timer_limit: int, symmetry: bool = True,
                        view: bool = True, invariants: Sequence[str] = ("AcknowledgedWriteNotLost",),
-                       client_count: int = 1, restart_empty_limit: int = 0) -> "ModelChecker":
+                       client_count: int = 1, restart_empty_limit: int = 0, property: bool = False,
+                       live_test_hooks: int = 0) -> "ModelChecker":
+        """property: check PROPERTY ViewChangeCompletes (as a cfg with SPECIFICATION Spec does).  live_test_hooks (tests):
+        1 = the liveness pass checks []<>Q, Q = "some replica's rep_commit_number >= 1", instead; 2 = in that pass every
+        state without successors steps to Init (include/vsr_b200.h, vsr_model_create)"""
         lib = load_library()
         h = C.c_void_p()
         err = C.create_string_buffer(1024)
         mask = 0
         for n in invariants:
             mask |= INVARIANT_BITS[n]
+        mask |= (512 if property else 0) | (1024 if live_test_hooks & 1 else 0) | (2048 if live_test_hooks & 2 else 0)
         rc = lib.vsr_model_create(replica_count, client_count, value_count, start_view_on_timer_limit, restart_empty_limit,
                                   int(symmetry), int(view), mask, C.byref(h), err, len(err))
         if rc:
@@ -410,6 +438,10 @@ class ModelChecker:
 
     def invariant(self, state: bytes) -> int:
         return int(self._lib.vsr_invariant(self._h, (C.c_uint8 * self.state_bytes).from_buffer_copy(state)))
+
+    def property_holds(self, state: bytes) -> bool:
+        """the state predicate the liveness pass checks (AllReplicasMoveToSameView, or the test hook's Q)"""
+        return bool(self._lib.vsr_property(self._h, (C.c_uint8 * self.state_bytes).from_buffer_copy(state)))
 
     def canon(self, state: bytes) -> bytes:
         b = (C.c_uint8 * self.state_bytes).from_buffer_copy(state)
@@ -508,7 +540,7 @@ class ModelChecker:
         """One-GPU BFS through the single C-ABI call ``vsr_bfs`` (counterexample included).  With collect_levels=True the
         same level loop, ``vsr_bfs_sharded``, runs on an engine held here, so that every level's states can be read back."""
         o = self.run_opts(**kw)
-        if o.collect_levels:
+        if o.collect_levels or self.info.property:
             return self._check_collecting(o)
         st = VsrStats()
         cap = 512
@@ -574,7 +606,8 @@ class ModelChecker:
         return [int(cands[i]) for i in range(n)], int(va.value)
 
     def _check_collecting(self, o: VsrRunOpts) -> CheckResult:
-        """``check(collect_levels=True)``: vsr_bfs_sharded on a world-1 engine, then every level's states read back."""
+        """``check(collect_levels=True)``, or a model with a PROPERTY: vsr_bfs_sharded on a world-1 engine, then every
+        level's states read back, and after a complete BFS the liveness pass (vsr_engine_liveness) with its lasso."""
         lib = self._lib
         e = C.c_void_p()
         err = C.create_string_buffer(512)
@@ -586,11 +619,11 @@ class ModelChecker:
             cap = 4096
             cands, n = (C.c_uint32 * cap)(), C.c_int(0)
             rc = lib.vsr_bfs_sharded(e, C.byref(o), 0, C.byref(st), cands, C.byref(n), cap)
-            if rc == 153:
+            if rc in (151, 153):
                 raise VsrError(rc, lib.vsr_engine_last_error(e).decode())
             levels = []
             sb = self.state_bytes
-            for lv in range(1, int(st.num_levels) + 1):
+            for lv in range(1, int(st.num_levels) + 1 if o.collect_levels else 1):
                 k = lib.vsr_engine_collected(e, lv, None, 0)
                 buf = (C.c_uint8 * (k * sb))()
                 lib.vsr_engine_collected(e, lv, buf, k)
@@ -598,6 +631,23 @@ class ModelChecker:
             trace = self._trace_from_cands(cands, n.value) if st.trace_len else []
             if rc == 12 and trace:
                 st.violation_mask = self.invariant(trace[-1][1])
-            return self.result_from_stats(st, rc, trace, levels)
+            live = {}
+            if rc == 0 and st.complete and self.info.property:
+                ls = VsrLiveStats()
+                rc = lib.vsr_engine_liveness(e, C.byref(ls), cands, cap)
+                if rc not in (0, 13):
+                    raise VsrError(rc, lib.vsr_engine_last_error(e).decode())
+                live = {k: getattr(ls, k) for k, _ in VsrLiveStats._fields_ if k != "_pad"}
+                live["ms_sweep"] = [float(ls.ms_sweep[i]) for i in range(min(int(ls.sweeps), VSR_MAX_SWEEPS))]
+                if rc == 13 and o.keep_trace:
+                    trace = self._trace_from_cands(cands, int(ls.trace_len))
+                    st.trace_loop = ls.trace_loop
+                    st.violation_level = ls.violation_level
+                if ls.error_code:
+                    st.error_code = ls.error_code
+            res = self.result_from_stats(st, rc, trace, levels)
+            res.liveness = live
+            res.trace_loop = int(st.trace_loop)
+            return res
         finally:
             lib.vsr_engine_destroy(e)

@@ -548,6 +548,26 @@ template <class L> struct Ops {
         return 0;
     }
 
+    /* AllReplicasMoveToSameView, VSR.tla:958-962: every replica is Normal and all have the same view number.  The state
+       predicate under ViewChangeCompletes == []<>AllReplicasMoveToSameView; reads only rep_status and rep_view_number */
+    template <class W> static VSR_HD bool all_same_view_normal(const RunCfg&, const W& w) {
+        const uint32_t v0 = VGET(L, VIEWN, w, 0);
+        for (int r = 0; r < R; r++)
+            if (VGET(L, STATUS, w, r) != 0 || VGET(L, VIEWN, w, r) != v0) return false;
+        return true;
+    }
+    /* test hook of the liveness pass (vsr_model_create only), not a spec predicate: "some replica has committed" — false
+       at Init, and some reachable states where it is false have no successor, so tests reach the violation paths */
+    template <class W> static VSR_HD bool some_commit(const W& w) {
+        for (int r = 0; r < R; r++)
+            if (VGET(L, COMMIT, w, r) >= 1) return true;
+        return false;
+    }
+    /* the predicate the liveness pass checks: P, or Q when the test hook (LIVE_HOOK_Q of vsr_model.h, bit 1) is on */
+    template <class W> static VSR_HD bool live_pred(const RunCfg& run, const W& w, int live_hooks) {
+        return (live_hooks & 1) ? some_commit(w) : all_same_view_normal(run, w);
+    }
+
     /* label-independent key of the aux variables for same-level VIEW ties (DESIGN.md §H2); same
        number the oracle's aux_key() computes */
     template <class W> static VSR_HD uint32_t aux_key(const W& w) {

@@ -12,10 +12,21 @@
 #include <sys/stat.h>
 #include <sys/types.h>
 
+#include <time.h>
+
+#include <chrono>
 #include <string>
 #include <vector>
 
 #include "../../include/vsr_b200.h"
+
+static double vsr_now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+static std::string vsr_clock_text() { /* TLC's "(2024-01-01 12:00:00)" time stamps */
+    char b[64];
+    const time_t t = time(nullptr);
+    strftime(b, sizeof b, "%Y-%m-%d %H:%M:%S", localtime(&t));
+    return b;
+}
 
 static void usage() {
     fprintf(stderr,
@@ -119,12 +130,60 @@ int main(int argc, char** argv) {
     if (!deadlock_flag && info.check_deadlock == 0) o.check_deadlock = 0; /* CHECK_DEADLOCK FALSE in the cfg, as in TLC */
     VsrStats st;
     memset(&st, 0, sizeof st);
-    const size_t tcap = 512;
+    const size_t tcap = 4096;
     std::vector<unsigned char> trace(tcap * (size_t)info.state_bytes);
     std::vector<uint8_t> acts(tcap);
     VsrSimStats sim;
     memset(&sim, 0, sizeof sim);
-    if (simulate) {
+    VsrLiveStats live;
+    memset(&live, 0, sizeof live);
+    const char* refused = !info.property ? nullptr
+                          : simulate ? "-simulate with PROPERTY ViewChangeCompletes: temporal properties are checked on the complete state graph only"
+                          : gpus > 1 ? "-gpus > 1 with PROPERTY ViewChangeCompletes: liveness on several GPUs is not supported"
+                          : (o.checkpoint_path || o.recover_path) ? "-checkpoint / -recover with PROPERTY ViewChangeCompletes: checkpointing the liveness store is not supported"
+                          : nullptr;
+    if (refused) {
+        fprintf(stderr, "Error: %s\n", refused);
+        vsr_model_free(m);
+        return VSR_RC_CONFIG_ERROR;
+    }
+    if (info.property && gpus == 1) {
+        /* one GPU: the BFS, then the liveness pass on the same engine (it keeps the store of not-P states) */
+        printf("Running breadth-first search Model-Checking with fp 0 on GPU %d.\n", o.device);
+        const double t0 = vsr_now_s();
+        VsrEngine* e = nullptr;
+        rc = vsr_engine_create(m, &o, 0, 1, &e, err, sizeof err);
+        if (rc) { fprintf(stderr, "Error: %s\n", err); vsr_model_free(m); return rc; }
+        std::vector<uint32_t> cands(tcap);
+        int n = 0;
+        rc = vsr_bfs_sharded(e, &o, 0, &st, cands.data(), &n, cands.size());
+        if (rc == VSR_RC_OK && st.complete) {
+            printf("Checking temporal properties for the complete state space with %llu total distinct states at (%s)\n", (unsigned long long)st.distinct,
+                   vsr_clock_text().c_str());
+            rc = vsr_engine_liveness(e, &live, cands.data(), cands.size());
+            n = live.trace_len;
+            if (rc == VSR_RC_LIVENESS) st.trace_len = o.keep_trace ? n + 1 : 0;
+            double sweep_ms = 0;
+            for (int i = 0; i < live.sweeps && i < VSR_MAX_SWEEPS; i++) sweep_ms += live.ms_sweep[i];
+            if (rc == VSR_RC_OK || rc == VSR_RC_LIVENESS)
+                printf("Liveness: %llu states where AllReplicasMoveToSameView is false stored (%.1f %% of %llu; %.2f GB in HBM, %.2f GB in host memory), "
+                       "%d sweeps in %.3f s of kernel time, %llu without successors, %llu on cycles\n",
+                       (unsigned long long)live.stored, st.distinct ? 100.0 * live.stored / st.distinct : 0.0, (unsigned long long)st.distinct,
+                       live.bytes_hbm / 1e9, live.bytes_host / 1e9, live.sweeps, sweep_ms * 1e-3, (unsigned long long)live.sinks,
+                       (unsigned long long)live.survivors);
+            if (rc == VSR_RC_OK) printf("Finished checking temporal properties in %.3f s at %s\n", live.seconds_total, vsr_clock_text().c_str());
+        } else if (rc == VSR_RC_OK) {
+            printf("Temporal properties were not checked: the search stopped before the state graph was complete "
+                   "(they are checked on the complete graph only).\n");
+        }
+        if ((rc == VSR_RC_VIOLATION || rc == VSR_RC_DEADLOCK || rc == VSR_RC_LIVENESS) && st.trace_len > 0) {
+            const int k = vsr_replay_candidates(m, cands.data(), n, trace.data(), acts.data(), tcap);
+            st.trace_len = k > 0 ? (k < (int)tcap ? k : (int)tcap) : 0;
+        }
+        if (rc && rc != VSR_RC_VIOLATION && rc != VSR_RC_DEADLOCK && rc != VSR_RC_LIVENESS) fprintf(stderr, "Error: %s\n", vsr_engine_last_error(e));
+        vsr_engine_destroy(e);
+        st.seconds_total = vsr_now_s() - t0;
+    } else if (simulate) {
         VsrSimOpts so;
         so.device = o.device;
         so.depth = o.max_depth > 0 ? o.max_depth : 100;
@@ -140,8 +199,10 @@ int main(int argc, char** argv) {
         rc = vsr_bfs_multi(m, &o, gpus, inbox_records, part_states, &st, trace.data(), acts.data(), tcap, err, sizeof err);
         if (err[0]) fprintf(stderr, "Error: %s\n", err);
     }
-    if (rc == VSR_RC_VIOLATION || rc == VSR_RC_DEADLOCK) {
-        if (rc == VSR_RC_VIOLATION) {
+    if (rc == VSR_RC_VIOLATION || rc == VSR_RC_DEADLOCK || rc == VSR_RC_LIVENESS) {
+        if (rc == VSR_RC_LIVENESS) {
+            printf("Error: Temporal properties were violated.\n");
+        } else if (rc == VSR_RC_VIOLATION) {
             /* which of the configured invariants the reported state violates: evaluated on that state (several may be configured) */
             int mask = st.violation_mask;
             if (!mask && st.trace_len > 0) mask = vsr_invariant(m, trace.data() + (size_t)(st.trace_len - 1) * info.state_bytes);
@@ -151,8 +212,9 @@ int main(int argc, char** argv) {
                 if (mask & (1 << b)) { printf("Error: Invariant %s is violated.\n", names[b]); any = true; }
             if (!any) printf("Error: Invariant is violated.\n");
         }
-        else printf("Error: Deadlock reached.\n");
-        printf("Error: The behavior up to this point is:\n");
+        else if (rc == VSR_RC_DEADLOCK) printf("Error: Deadlock reached.\n");
+        if (rc == VSR_RC_LIVENESS) printf("Error: The following behavior constitutes a counter-example:\n");
+        else printf("Error: The behavior up to this point is:\n");
         std::vector<char> buf(1 << 18);
         std::string dumptext = "<<\n";
         for (int i = 0; i < st.trace_len; i++) {
@@ -166,6 +228,19 @@ int main(int argc, char** argv) {
                         "\",\n   location |-> \"" + loc + "\"\n ],\n" + buf.data() + "]" + (i + 1 < st.trace_len ? ",\n" : "\n");
         }
         dumptext += ">>";
+        if (rc == VSR_RC_LIVENESS && st.trace_len > 0) { /* the lasso's end: a step back into the behaviour, or stuttering forever */
+            std::string tail;
+            if (live.trace_loop > 0) {
+                char loc[128];
+                vsr_action_location(m, live.trace_loop_action, loc, sizeof loc);
+                tail = std::to_string(st.trace_len + 1) + ": Back to state " + std::to_string(live.trace_loop) + ": <" +
+                       vsr_action_name(live.trace_loop_action) + " " + loc + ">";
+            } else {
+                tail = std::to_string(st.trace_len + 1) + ": Stuttering";
+            }
+            printf("%s\n", tail.c_str());
+            dumptext += "\n\\* " + tail + "\n";
+        }
         if (dump) {
             FILE* f = fopen(dump, "w");
             if (f) { fputs(dumptext.c_str(), f); fclose(f); printf("Trace written to %s\n", dump); }

@@ -73,10 +73,29 @@ struct VsrEngine {
     double level_ms_insert_acc = 0; /* the part of level_ms_acc spent in launches that only insert records from peers */
     uint64_t records_sent = 0, records_received = 0;
     std::vector<std::vector<uint8_t>> collected; /* per level states (collect_levels) */
+    /* liveness store (models with a property; vsr_live.cu): the not-P states of every finished level, grouped by level */
+    uint32_t* live_words = nullptr;      /* [0, live_dev_cap) in HBM */
+    uint32_t* live_words_host = nullptr; /* the rest in pinned host memory mapped into the device */
+    uint64_t live_cap = 0, live_dev_cap = 0;
+    unsigned long long* live_ids = nullptr; /* BFS local id per stored state */
+    uint64_t* live_index = nullptr;      /* {fp, (store index + 1) << 32 | check} */
+    uint64_t live_index_cap = 0;
+    uint32_t* live_alive = nullptr;      /* one bit per store index */
+    vsr::LiveCtr* live_ctr = nullptr;
+    std::vector<uint64_t> live_level_off; /* live_level_off[d - 1] = store index of depth d's first state; back() = stored */
+    uint64_t live_bytes_hbm = 0, live_bytes_host = 0;
     char last_error[256] = {0};
 };
 
 int engine_reset_level(VsrEngine* e);
 void fill_params(VsrEngine* e, vsr::ExpandParams& p);
+/* vsr_live.cu: the liveness store's allocation (after the BFS's, from what memory is left), release, clearing, and the
+   per-level collection vsr_engine_finish_level calls for a model with a property */
+int live_create(VsrEngine* e, char* err, size_t errcap);
+void live_destroy(VsrEngine* e);
+int live_reset(VsrEngine* e);
+int live_collect(VsrEngine* e);
+/* vsr_shard.cu: the candidate chain from Init to global state id `gid` (every rank of a group calls it together) */
+int walk_trace(VsrEngine* e, uint64_t gid, std::vector<uint32_t>& cands);
 
 #endif

@@ -123,6 +123,8 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     if (!m->gpu) return fail(VSR_RC_CONFIG_ERROR, "no GPU kernels compiled for this configuration");
     if (world < 1 || world > MAX_WORLD || (world & (world - 1)) || rank < 0 || rank >= world)
         return fail(VSR_RC_CONFIG_ERROR, "world must be 1, 2, 4 or 8 and 0 <= rank < world");
+    if (m->info.property && world > 1)
+        return fail(VSR_RC_CONFIG_ERROR, "PROPERTY ViewChangeCompletes is checked on one GPU only: liveness on several GPUs is not supported");
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
     if (ce != cudaSuccess || ndev == 0)
@@ -165,9 +167,12 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     cudaMemGetInfo(&free_b, &total_b);
     uint64_t tcap = opts->table_capacity, fcap = opts->frontier_capacity;
     const uint64_t S = (uint64_t)e->g->bytes;
-    if (!tcap) tcap = (uint64_t)(free_b * 0.45) / 23; /* table 16 B/slot + trace 8 B per state at load <= 7/8  ->  23 B per slot; ~45% of free memory */
+    /* with a property the liveness store takes what the BFS leaves: its live index (2 slots of 16 B per stored state) is
+       about as large again as the seen-set and the trace, so the automatic sizes leave it more than half of the memory */
+    const bool live = m->info.property != 0;
+    if (!tcap) tcap = (uint64_t)(free_b * (live ? 0.25 : 0.45)) / 23; /* table 16 B/slot + trace 8 B per state at load <= 7/8  ->  23 B per slot; ~45% of free memory */
     tcap = (tcap + 63) & ~63ull; /* any size (whole buckets / cache lines), not only powers of two */
-    if (!fcap) fcap = (uint64_t)(free_b * 0.40) / (2 * S);
+    if (!fcap) fcap = (uint64_t)(free_b * (live ? 0.15 : 0.40)) / (2 * S);
     if (fcap < 64) fcap = 64;
     e->table_cap = tcap;
     e->frontier_cap = fcap;
@@ -195,6 +200,13 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     e->st.bytes_frontier = 2 * fcap * S;
     e->st.bytes_h2d += 8 * 256 * 8;
     if ((ce = cudaStreamSynchronize(e->stream)) != cudaSuccess) return bail("sync", ce);
+    if (live) {
+        const int rc = live_create(e, err, errcap);
+        if (rc) {
+            vsr_engine_destroy(e);
+            return rc;
+        }
+    }
     *out = e;
     return 0;
 }
@@ -211,6 +223,7 @@ void vsr_engine_destroy(VsrEngine* e) {
     if (e->stream) cudaFreeAsync(e->ties, e->stream); else cudaFree(e->ties);
     if (e->stream) cudaFreeAsync(e->fp_tab, e->stream); else cudaFree(e->fp_tab);
     if (e->stream) cudaFreeAsync(e->init_rec, e->stream); else cudaFree(e->init_rec);
+    live_destroy(e);
     vsr_engine_detach(e);
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
@@ -435,6 +448,11 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
     e->next_base += n_new;
     e->level = gen_level;
     e->level_open = false;
+    if (e->live_index && !li.overflow) { /* the property's store: this level's not-P states */
+        const int rc = live_collect(e);
+        if (rc == VSR_RC_TOO_LARGE) li.overflow = 5;
+        else if (rc) return rc;
+    }
     if (e->opts.collect_levels) { /* one entry per level, empty when this rank found nothing at that depth (several ranks) */
         std::vector<uint8_t> host((size_t)n_new * e->g->bytes);
         if (n_new && vsr_engine_read_frontier(e, 0, n_new, host.data())) return VSR_RC_SYSTEM;
@@ -533,7 +551,7 @@ int vsr_engine_reset(VsrEngine* e) {
     e->cur = 0; e->n_cur = 0; e->cur_base = 0; e->next_base = 0; e->level = 0; e->level_open = false;
     e->records_sent = e->records_received = 0;
     e->collected.clear();
-    return 0;
+    return live_reset(e);
 }
 
 int vsr_engine_stats(const VsrEngine* e, VsrStats* out) {
@@ -558,6 +576,7 @@ int vsr_simulate(const VsrModel* m, const VsrSimOpts* o, VsrSimStats* out, void*
     if (!m || !o || !out) return VSR_RC_ERROR;
     memset(out, 0, sizeof *out);
     if (!m->gpu) return VSR_RC_CONFIG_ERROR;
+    if (m->info.property) return out->rc = VSR_RC_CONFIG_ERROR; /* a random walk cannot decide []<>P: temporal properties need the whole graph */
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return VSR_RC_SYSTEM;
     if (cudaSetDevice(o->device) != cudaSuccess) return VSR_RC_SYSTEM;
@@ -673,3 +692,7 @@ int vsr_probe_bench(int device, uint64_t capacity, uint64_t n, double dup_frac, 
 }
 
 } /* extern "C" */
+
+/* the liveness pass is part of this translation unit: the library's sources stay the four the single-layout builds of
+   the tests and tools compile (vsr_gpu.cu, vsr_shard.cu, vsr_ckpt.cu, vsr_host.cpp) */
+#include "vsr_live.cu"

@@ -6,6 +6,7 @@
 #define VSR_GPU_THUNKS_CUH
 
 #include "vsr_gpu.cuh"
+#include "vsr_live.cuh"
 #include "vsr_model.h"
 
 namespace vsr {
@@ -23,6 +24,9 @@ struct GpuOps {
     /* the expand kernel's shape (ExpandCfg): warps per block, blocks per SM, scan passes per round, staging rows per warp */
     int warps, blocks, passes, stage_rows;
     cudaError_t (*launch_audit)(const ExpandParams&, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t);
+    /* liveness pass (vsr_live.cuh): store a level's not-P states; one elimination sweep over store indices [first, first + n) */
+    cudaError_t (*launch_live_collect)(const LiveParams&, int sms, cudaStream_t);
+    cudaError_t (*launch_live_sweep)(const LiveParams&, int sms, cudaStream_t);
 };
 
 /* what a layout plug-in must have been compiled against: the version constant AND the shapes of the structs the kernels and the
@@ -62,12 +66,25 @@ template <class L> struct GpuThunks {
         if (n_states) audit_frontier_kernel<L><<<sms * 8, 256, 0, st>>>(p, n_states, out);
         return cudaGetLastError();
     }
+    static cudaError_t launch_live_collect(const LiveParams& q, int sms, cudaStream_t st) {
+        if (!q.n_in) return cudaSuccess;
+        const unsigned long long want = (q.n_in + 255) / 256, most = (unsigned long long)sms * 8;
+        live_collect_kernel<L><<<(unsigned)(want < most ? want : most), 256, 0, st>>>(q);
+        return cudaGetLastError();
+    }
+    static cudaError_t launch_live_sweep(const LiveParams& q, int sms, cudaStream_t st) {
+        if (!q.n) return cudaSuccess;
+        const unsigned long long want = (q.n + 127) / 128, most = (unsigned long long)sms * 16;
+        live_sweep_kernel<L><<<(unsigned)(want < most ? want : most), 128, 0, st>>>(q);
+        return cudaGetLastError();
+    }
     static uint32_t chk(const uint32_t* w, int use_view) { return check_hash<L>(w, use_view != 0); }
     static const GpuOps* get() {
         typedef ExpandCfg<L> Cfg;
         static const GpuOps ops = {chk, L::R, L::V, L::K, L::NW, L::BYTES, (int)(L::BYTES + sizeof(RecHdr)), sizeof(typename Cfg::Smem), Cfg::WARPS * 32,
                                    launch_expand, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate,
-                                   Cfg::WARPS, Cfg::BLOCKS, Cfg::PASSES, Expander<L, false>::SROWS, launch_audit};
+                                   Cfg::WARPS, Cfg::BLOCKS, Cfg::PASSES, Expander<L, false>::SROWS, launch_audit,
+                                   launch_live_collect, launch_live_sweep};
         return &ops;
     }
 };

@@ -372,6 +372,7 @@ static int parse_cfg(const std::string& text, VsrModel* m, std::string& why) {
     bool have_values = false;
     std::string init, next, view, symm, spec;
     std::vector<std::string> invs;
+    std::vector<Tok> props;
     m->check_deadlock_cfg = -1;
     auto at = [&](size_t i) -> std::string { return i < t.size() ? t[i].s : std::string(); };
     auto where = [&](size_t i) { return " (cfg line " + std::to_string(i < t.size() ? t[i].line : (t.empty() ? 0 : t.back().line)) + ")"; };
@@ -415,11 +416,15 @@ static int parse_cfg(const std::string& text, VsrModel* m, std::string& why) {
             m->check_deadlock_cfg = at(i + 1) == "TRUE" ? 1 : 0;
             i += 2;
         } else if (k == "SPECIFICATION") {
-            /* Spec == Init /\ [][Next]_vars /\ WF_vars(Next) (VSR.tla:966): for invariant checking TLC explores Init/Next
-               exactly as with INIT/NEXT; the fairness conjunct only matters to PROPERTY formulas, which are refused below */
+            /* Spec == Init /\ [][Next]_vars /\ WF_vars(Next) (VSR.tla:967): for invariant checking TLC explores Init/Next
+               exactly as with INIT/NEXT; the fairness conjunct is what PROPERTY ViewChangeCompletes is checked under */
             spec = at(i + 1);
             i += 2;
-        } else if (k == "PROPERTY" || k == "PROPERTIES" || k == "CONSTRAINT" || k == "CONSTRAINTS" ||
+        } else if (k == "PROPERTY" || k == "PROPERTIES") {
+            i++;
+            if (i >= t.size() || is_keyword(t[i].s)) { why = "`" + k + "` names no property" + where(i); return VSR_RC_CONFIG_ERROR; }
+            while (i < t.size() && !is_keyword(t[i].s)) props.push_back({t[i].s, t[i].line}), i++;
+        } else if (k == "CONSTRAINT" || k == "CONSTRAINTS" ||
                    k == "ACTION_CONSTRAINT" || k == "ACTION_CONSTRAINTS" || k == "POSTCONDITION" || k == "ALIAS") {
             why = "`" + k + "` is not supported: this checker runs safety (invariant) checking of VSR.tla only (no temporal "
                   "formulas, liveness or constraints)" + where(i);
@@ -436,6 +441,23 @@ static int parse_cfg(const std::string& text, VsrModel* m, std::string& why) {
     for (size_t a = 0; a < values.size(); a++)
         for (size_t b = a + 1; b < values.size(); b++)
             if (values[a] == values[b]) { why = "duplicate element `" + values[a] + "` in Values"; return VSR_RC_CONFIG_ERROR; }
+    int property = 0;
+    for (const Tok& p : props) {
+        if (p.s != "ViewChangeCompletes") {
+            why = "PROPERTY `" + p.s + "` is not supported: the one temporal property checked is ViewChangeCompletes (VSR.tla:964-965)" +
+                  (p.s == "AllReplicasMoveToSameView" ? std::string("; AllReplicasMoveToSameView is its state predicate, not a temporal formula") : std::string()) +
+                  " (cfg line " + std::to_string(p.line) + ")";
+            return VSR_RC_CONFIG_ERROR;
+        }
+        property |= 1;
+    }
+    if (property && spec.empty()) {
+        /* under [][Next]_vars alone stuttering at the first not-P state violates []<>P trivially: the property is only
+           meaningful with the fairness conjunct of Spec */
+        why = "PROPERTY ViewChangeCompletes needs `SPECIFICATION Spec` (VSR.tla:967: Spec's WF_vars(Next) is what makes it "
+              "meaningful); with INIT/NEXT and no fairness it is refused";
+        return VSR_RC_CONFIG_ERROR;
+    }
     if (!spec.empty()) {
         if (!init.empty() || !next.empty()) { why = "the config names both SPECIFICATION and INIT/NEXT (TLC refuses that too)"; return VSR_RC_CONFIG_ERROR; }
         if (spec != "Spec") { why = "SPECIFICATION `" + spec + "` unknown; VSR.tla defines `Spec` (:966)"; return VSR_RC_CONFIG_ERROR; }
@@ -463,6 +485,7 @@ static int parse_cfg(const std::string& text, VsrModel* m, std::string& why) {
     I.symmetry = symm.empty() ? 0 : 1;
     I.view = view.empty() ? 0 : 1;
     I.invariant = mask;
+    I.property = property;
     for (size_t v = 0; v < values.size() && v < VSR_MAX_V; v++) snprintf(I.value_names[v], sizeof I.value_names[v], "%s", values[v].c_str());
     return 0;
 }
@@ -800,7 +823,10 @@ int vsr_model_create(int R, int C, int V, int L, int restart, int symmetry, int 
     m->check_deadlock_cfg = -1;
     VsrModelInfo& I = m->info;
     I.replica_count = R; I.client_count = C; I.value_count = V; I.start_view_on_timer_limit = L; I.restart_empty_limit = restart;
-    I.symmetry = symmetry ? 1 : 0; I.view = view ? 1 : 0; I.invariant = invariant;
+    I.symmetry = symmetry ? 1 : 0; I.view = view ? 1 : 0;
+    I.invariant = invariant & ~(MODEL_PROPERTY_BIT | MODEL_HOOK_Q_BIT | MODEL_HOOK_INIT_EDGE_BIT);
+    I.property = (invariant & MODEL_PROPERTY_BIT) ? 1 : 0;
+    m->live_hooks = ((invariant & MODEL_HOOK_Q_BIT) ? LIVE_HOOK_Q : 0) | ((invariant & MODEL_HOOK_INIT_EDGE_BIT) ? LIVE_HOOK_INIT_EDGE : 0);
     if (V < 1 || V > VSR_MAX_V) { set_err(err, errcap, "|Values| out of range"); delete m; return VSR_RC_CONFIG_ERROR; }
     for (int v = 0; v < V; v++) snprintf(I.value_names[v], sizeof I.value_names[v], "v%d", v + 1);
     return finish_load(m, nullptr, out, err, errcap);
@@ -866,6 +892,7 @@ int vsr_owner_rank(uint64_t fingerprint, int world) {
     return vsr::owner_of(fingerprint ? fingerprint : 1, 64 - lg);
 }
 int vsr_invariant(const VsrModel* m, const void* s) { return m->ops->invariant(&m->run, (const uint32_t*)s); }
+int vsr_property(const VsrModel* m, const void* s) { return m->ops->property(&m->run, (const uint32_t*)s, m->live_hooks); }
 int vsr_unpack(const VsrModel* m, const void* s, VsrFlatState* out) { return m->ops->unpack((const uint32_t*)s, out); }
 int vsr_pack(const VsrModel* m, const VsrFlatState* in, void* s) { return m->ops->pack(in, (uint32_t*)s, m->run.symmetry); }
 

@@ -64,7 +64,10 @@ enum {
     E_STALE_RECV = -4,      /* SendGetState with non-empty received sets: their view would go stale */
     E_PREPKEY_CLASH = -5,   /* two created values share (view, op_number): canonical labelling undefined */
     E_MISSING_PAYLOAD = -6, /* a received DVC whose slot is absent */
-    E_UNSUPPORTED = -7      /* state not representable (pack): restart variables, count > 1, ... */
+    E_UNSUPPORTED = -7,     /* state not representable (pack): restart variables, count > 1, ... */
+    /* liveness pass (vsr_live.cu): the BFS and the store of not-P states disagree */
+    E_LIVE_MISSING = -8,    /* a not-P successor of a stored state is not in the live index */
+    E_LIVE_DUP = -9         /* a state was stored twice */
 };
 
 #define VSR_FIELD(name, W, N, prev)                           \

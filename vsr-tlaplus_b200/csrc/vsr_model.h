@@ -24,6 +24,10 @@ namespace vsr {
 
 struct GpuOps; /* vsr_gpu.cu */
 
+/* vsr_model_create's `invariant` bits above the INVARIANT mask (include/vsr_b200.h) */
+enum { MODEL_PROPERTY_BIT = 512, MODEL_HOOK_Q_BIT = 1024, MODEL_HOOK_INIT_EDGE_BIT = 2048 };
+enum { LIVE_HOOK_Q = 1, LIVE_HOOK_INIT_EDGE = 2 };
+
 struct ModelOps {
     int R, V, K, nw, bytes, bits, ncand;
     void (*init)(uint32_t*);
@@ -40,9 +44,10 @@ struct ModelOps {
     uint64_t (*fingerprint_bytewise)(const uint32_t*, int use_view);
     int (*random_enabled)(const RunCfg*, const uint32_t*, uint64_t* rng);
     int (*enabled_list)(const RunCfg*, const uint32_t*, uint32_t* out); /* register-mask form of the guards (the kernel's scan) */
+    int (*property)(const RunCfg*, const uint32_t*, int live_hooks);   /* the liveness pass's state predicate (live_pred) */
 };
 /* bump when ModelOps / GpuOps / ExpandParams change shape: a layout plug-in built against another value is rebuilt */
-#define VSR_PLUGIN_ABI 6
+#define VSR_PLUGIN_ABI 7
 const ModelOps* find_model_ops(int R, int V, int K);
 const GpuOps* find_gpu_ops(int R, int V, int K); /* defined in vsr_gpu.cu */
 
@@ -56,6 +61,7 @@ struct VsrModel {
     const vsr::ModelOps* ops;
     const vsr::GpuOps* gpu;
     int check_deadlock_cfg; /* CHECK_DEADLOCK in the cfg: -1 unset */
+    int live_hooks = 0;     /* test hooks of the liveness pass (vsr_model_create): LIVE_HOOK_* */
     std::string action_location[VSR_NUM_ACTIONS];
 };
 

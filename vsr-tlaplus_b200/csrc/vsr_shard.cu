@@ -63,6 +63,8 @@ int set_error(VsrEngine* e, const char* fmt, const char* a = "") {
     return VSR_RC_SYSTEM;
 }
 
+} // namespace
+
 /* The candidate chain from Init to state `gid` (rank << 40 | local id), from the (parent, candidate) trace records.  With
    several ranks the owner of each record shares it in an all-gather: every rank calls this with the same gid. */
 int walk_trace(VsrEngine* e, uint64_t gid, std::vector<uint32_t>& cands) {
@@ -93,6 +95,8 @@ int walk_trace(VsrEngine* e, uint64_t gid, std::vector<uint32_t>& cands) {
     std::reverse(cands.begin(), cands.end());
     return 0;
 }
+
+namespace {
 
 /* The counterexample of the one-call APIs: the candidate chain vsr_bfs_sharded walked (stats->trace_len > 0: it did)
    replayed into literal states; a violation reports the invariants its last state violates. */
@@ -234,6 +238,10 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     if (trace_len) *trace_len = 0;
     VsrGroup* g = e->group;
     if (e->world > 1 && (!g || !e->inbox || e->stage)) return set_error(e, "vsr_bfs_sharded needs vsr_engine_attach_group first");
+    if (e->m->info.property && (opts->checkpoint_path || opts->recover_path)) {
+        snprintf(e->last_error, sizeof e->last_error, "-checkpoint / -recover with PROPERTY ViewChangeCompletes: checkpointing the liveness store is not supported");
+        return VSR_RC_CONFIG_ERROR;
+    }
     const int W = e->world, me = e->rank;
     const double t0 = now_s();
     /* a step of S states per rank fills each peer segment with about S * (successor records per state) / W records.  The
@@ -542,6 +550,17 @@ int vsr_bfs(const VsrModel* m, const VsrRunOpts* opts, VsrStats* stats, void* tr
     int n = 0;
     rc = vsr_bfs_sharded(e, opts, 0, stats, trace_out ? cands.data() : nullptr, &n, cands.size());
     replay_counterexample(m, rc, cands.data(), n, stats, trace_out, trace_actions, trace_cap);
+    if (rc == VSR_RC_OK && stats->complete && m->info.property) { /* the temporal property, on the complete graph */
+        VsrLiveStats ls;
+        rc = vsr_engine_liveness(e, &ls, cands.data(), cands.size());
+        if (rc == VSR_RC_LIVENESS) {
+            stats->trace_len = e->trace ? ls.trace_len + 1 : 0; /* > 0: a lasso was walked, replay it */
+            replay_counterexample(m, rc, cands.data(), ls.trace_len, stats, trace_out, trace_actions, trace_cap);
+            stats->trace_loop = ls.trace_loop;
+            stats->violation_level = ls.violation_level;
+        }
+        if (ls.error_code) stats->error_code = ls.error_code;
+    }
     stats->rc = rc;
     stats->seconds_setup = t_setup;
     stats->seconds_total = now_s() - t0;

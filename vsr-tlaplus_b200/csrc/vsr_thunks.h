@@ -33,9 +33,11 @@ template <class L> struct Thunks {
     static int unpack(const uint32_t* w, VsrFlatState* f) { return Conv<L>::unpack(w, f); }
     static int pack(const VsrFlatState* f, uint32_t* w, int sym) { return Conv<L>::pack(f, w, sym != 0); }
     static int literal_cand(const uint32_t* w, int cand) { return Ops<L>::literal_cand(w, cand); }
+    static int property(const RunCfg* run, const uint32_t* w, int live_hooks) { return Ops<L>::live_pred(*run, w, live_hooks) ? 1 : 0; }
     static const ModelOps* get() {
         static const ModelOps ops = {L::R, L::V, L::K, L::NW, L::BYTES, L::TOTAL_BITS, L::NCAND, init, step, guard,
-                                     action_of, invariant, fingerprint, aux_key, canon, unpack, pack, literal_cand, fingerprint_bytewise, random_enabled, enabled_list};
+                                     action_of, invariant, fingerprint, aux_key, canon, unpack, pack, literal_cand, fingerprint_bytewise, random_enabled, enabled_list,
+                                     property};
         return &ops;
     }
 };
