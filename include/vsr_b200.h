@@ -109,6 +109,23 @@ const char* vsr_action_name(int action_id);
 int vsr_action_location(const VsrModel* m, int action_id, char* buf, size_t cap);
 
 /* ---- the BFS (TLC's worker loop; SURVEY §3.1, stages E1-E9) on the GPU */
+#define VSR_MAX_LEVELS 512
+/* Action coverage, TLC's `-coverage`: per action of Next (VSR_ACT_*; 0 = the initial predicate) and per BFS level d
+ * (depth of the SUCCESSOR, Init = 1; row d - 1):
+ *   generated  sum of mult over the successors produced by a binding of that action: TLC's "states generated", one per
+ *              binding.  Deterministic, and the same for every number of GPUs.
+ *   distinct   states whose first arrival in the seen-set came through that action (after a same-level VIEW tie was
+ *              resolved with parent records kept: the surviving arrival's action, as in the trace).  A state reachable
+ *              in one level through two actions goes to whichever insert won, so the split over actions may differ
+ *              from run to run; its sum per level is the level's size.
+ * num_levels = rows in use: a complete run whose deepest level has successors has depth + 1, the last one holding those
+ * successors, all of them seen before.  Counted by the expand kernel where a state is inserted, on the GPU that owns it. */
+typedef struct VsrCoverage {
+    uint64_t generated[VSR_NUM_ACTIONS], distinct[VSR_NUM_ACTIONS];
+    int32_t num_levels, _pad;
+    uint64_t level_generated[VSR_MAX_LEVELS][VSR_NUM_ACTIONS], level_distinct[VSR_MAX_LEVELS][VSR_NUM_ACTIONS];
+} VsrCoverage;
+
 typedef struct VsrRunOpts {
     int32_t device;              /* CUDA device ordinal */
     int32_t check_deadlock;      /* TLC default is on; `-deadlock` turns it off.  Here default 0 (VSR has terminal states) */
@@ -134,9 +151,13 @@ typedef struct VsrRunOpts {
     const char* checkpoint_path;
     const char* recover_path;
     double checkpoint_seconds;
+    /* action coverage: NULL = off (the kernels are launched without the counters).  Else the BFS counts, and
+       vsr_bfs_sharded (vsr_bfs, vsr_bfs_multi) writes the job's totals here when it returns, however the run ended; an
+       engine created with it set counts in the stepwise interface too (vsr_engine_coverage).  Refused (151) together
+       with checkpoint_path / recover_path: the counters are not in the checkpoint file. */
+    VsrCoverage* coverage;
 } VsrRunOpts;
 
-#define VSR_MAX_LEVELS 512
 typedef struct VsrStats {
     uint64_t generated, distinct, queue;  /* TLC's "N states generated, M distinct states found, Q left on queue" */
     int32_t depth;                        /* TLC's "depth of the complete state graph search" (Init = 1) */
@@ -229,6 +250,8 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out);
 /* forget everything explored (clears the seen-set, keeps the allocations): ready for seed_init again */
 int vsr_engine_reset(VsrEngine* e);
 const char* vsr_engine_last_error(const VsrEngine* e);
+/* THIS rank's action coverage of the levels finished so far (engines created with opts.coverage set; else 151) */
+int vsr_engine_coverage(const VsrEngine* e, VsrCoverage* out);
 /* with opts.collect_levels: number of states first seen at depth `level` (1-based) and, if host_out has room, a copy */
 uint64_t vsr_engine_collected(const VsrEngine* e, int level, void* host_out, uint64_t cap_states);
 /* Audit of the level just finished (tests): one device pass over this rank's seen-set and current frontier.
@@ -355,6 +378,9 @@ int vsr_walk(const VsrModel* m, uint64_t seed, uint64_t walk, int depth, uint32_
 int vsr_probe_bench(int device, uint64_t capacity, uint64_t n, double dup_frac, int iters, double* out);
 
 const char* vsr_version(void);
+/* sizeof of an ABI struct by name ("VsrRunOpts", "VsrCoverage", "VsrStats", "VsrLevelInfo"; 0 = unknown), for bindings that
+ * mirror the structs to check themselves against */
+size_t vsr_sizeof(const char* struct_name);
 
 #ifdef __cplusplus
 }

@@ -10,6 +10,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from collections import OrderedDict
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Tuple
 
@@ -90,6 +91,15 @@ class VsrModelInfo(C.Structure):
     ]
 
 
+class VsrCoverage(C.Structure):
+    _fields_ = [
+        ("generated", C.c_uint64 * VSR_NUM_ACTIONS), ("distinct", C.c_uint64 * VSR_NUM_ACTIONS),
+        ("num_levels", C.c_int32), ("_pad", C.c_int32),
+        ("level_generated", (C.c_uint64 * VSR_NUM_ACTIONS) * VSR_MAX_LEVELS),
+        ("level_distinct", (C.c_uint64 * VSR_NUM_ACTIONS) * VSR_MAX_LEVELS),
+    ]
+
+
 class VsrRunOpts(C.Structure):
     _fields_ = [
         ("device", C.c_int32), ("check_deadlock", C.c_int32), ("max_depth", C.c_int32),
@@ -97,7 +107,7 @@ class VsrRunOpts(C.Structure):
         ("table_capacity", C.c_uint64), ("frontier_capacity", C.c_uint64), ("max_states", C.c_uint64),
         ("max_seconds", C.c_double), ("collect_levels", C.c_int32), ("_reserved0", C.c_int32),
         ("frontier_host_capacity", C.c_uint64), ("checkpoint_path", C.c_char_p), ("recover_path", C.c_char_p),
-        ("checkpoint_seconds", C.c_double),
+        ("checkpoint_seconds", C.c_double), ("coverage", C.POINTER(VsrCoverage)),
     ]
 
 
@@ -171,7 +181,7 @@ EXPORTED_SYMBOLS = [
     "vsr_group_open", "vsr_group_open_local", "vsr_group_close", "vsr_group_barrier", "vsr_group_allgather", "vsr_group_abort",
     "vsr_group_set_timeout", "vsr_group_rank", "vsr_group_world", "vsr_group_last_error",
     "vsr_engine_attach_group", "vsr_engine_attach_staged", "vsr_engine_detach", "vsr_engine_default_inbox_records",
-    "vsr_bfs_sharded", "vsr_bfs_multi", "vsr_engine_liveness",
+    "vsr_bfs_sharded", "vsr_bfs_multi", "vsr_engine_liveness", "vsr_engine_coverage", "vsr_sizeof",
 ]
 
 _lib = None
@@ -254,6 +264,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.vsr_engine_lookup.argtypes = [vp, vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.vsr_engine_last_error.argtypes = [vp]
     lib.vsr_engine_last_error.restype = cp
+    lib.vsr_engine_coverage.argtypes = [vp, C.POINTER(VsrCoverage)]
+    lib.vsr_sizeof.argtypes = [cp]
+    lib.vsr_sizeof.restype = C.c_size_t
     lib.vsr_engine_collected.argtypes = [vp, C.c_int, vp, u64]
     lib.vsr_engine_collected.restype = u64
     lib.vsr_engine_build_trace.argtypes = [vp, u64, vp, C.POINTER(C.c_uint8), C.c_size_t]
@@ -293,6 +306,29 @@ def cfg_text(replica_count: int, values: Sequence[str], start_view_on_timer_limi
 
 
 @dataclass
+class Coverage:
+    """TLC's action coverage (`-coverage`; include/vsr_b200.h VsrCoverage).  by_action: action name (ACTION_NAMES order) ->
+    (distinct, generated).  levels = (distinct, generated): two uint64 arrays of shape [rows, 20], row d - 1 = successors of
+    depth d; a complete run whose deepest level has successors has depth + 1 rows (the last: those successors, all seen before)."""
+    by_action: "OrderedDict[str, Tuple[int, int]]"
+    levels: tuple
+
+    @classmethod
+    def from_struct(cls, cov: "VsrCoverage") -> "Coverage":
+        import numpy as np
+        n = int(cov.num_levels)
+        gen = np.ctypeslib.as_array(cov.level_generated)[:n].astype(np.uint64)
+        dis = np.ctypeslib.as_array(cov.level_distinct)[:n].astype(np.uint64)
+        return cls(OrderedDict((ACTION_NAMES[a], (int(cov.distinct[a]), int(cov.generated[a]))) for a in range(VSR_NUM_ACTIONS)),
+                   (dis, gen))
+
+    @property
+    def never_enabled(self) -> List[str]:
+        """lowered actions (not the four recovery actions, which need RestartEmptyLimit > 0) that generated nothing"""
+        return [n for n in ACTION_NAMES[1:16] if self.by_action[n][1] == 0]
+
+
+@dataclass
 class CheckResult:
     """What a TLC run reports (SURVEY §5 'Metrics'): the four scalars, the verdict, the trace."""
     rc: int
@@ -327,6 +363,7 @@ class CheckResult:
     # lasso's "Back to state K" (1-based into `trace`; 0 = the lasso ends in stuttering)
     liveness: dict = field(default_factory=dict)
     trace_loop: int = 0
+    coverage: Optional[Coverage] = None  # check(coverage=True): TLC's action coverage; None when it was not asked for
 
     @property
     def violated(self) -> bool:
@@ -497,10 +534,13 @@ class ModelChecker:
                  frontier_capacity: int = 0, keep_trace: bool = True, collect_levels: bool = False, max_states: int = 0,
                  max_seconds: float = 0.0, stop_on_violation: bool = True, verbose: bool = False,
                  frontier_host_capacity: int = 0, checkpoint_path: Optional[str] = None, recover_path: Optional[str] = None,
-                 checkpoint_seconds: float = 0.0) -> VsrRunOpts:
+                 checkpoint_seconds: float = 0.0, coverage: bool = False) -> VsrRunOpts:
         """checkpoint_path / recover_path / checkpoint_seconds: TLC's -checkpoint / -recover (a file per rank at level
-        boundaries; see include/vsr_b200.h VsrRunOpts)"""
+        boundaries; see include/vsr_b200.h VsrRunOpts).  coverage: count TLC's action coverage (CheckResult.coverage)"""
         o = VsrRunOpts()
+        if coverage:
+            o.cov = VsrCoverage()  # kept alive by the options object
+            o.coverage = C.pointer(o.cov)
         o.device = device
         if deadlock is None:  # CHECK_DEADLOCK of the cfg when it has one; otherwise off (VSR.tla has terminal states)
             deadlock = int(self.info.check_deadlock) == 1
@@ -536,6 +576,10 @@ class ModelChecker:
             records_sent=int(st.records_sent), records_received=int(st.records_received), seconds_insert=float(st.seconds_insert),
             trace=trace or [], levels=levels or [])
 
+    @staticmethod
+    def _coverage_of(o: VsrRunOpts) -> Optional[Coverage]:
+        return Coverage.from_struct(o.cov) if o.coverage else None
+
     def check(self, **kw) -> CheckResult:
         """One-GPU BFS through the single C-ABI call ``vsr_bfs`` (counterexample included).  With collect_levels=True the
         same level loop, ``vsr_bfs_sharded``, runs on an engine held here, so that every level's states can be read back."""
@@ -552,7 +596,9 @@ class ModelChecker:
         raw = bytes(tr)
         sb = self.state_bytes
         trace = [(ACTION_NAMES[acts[i]], raw[i * sb:(i + 1) * sb]) for i in range(int(st.trace_len))]
-        return self.result_from_stats(st, rc, trace)
+        res = self.result_from_stats(st, rc, trace)
+        res.coverage = self._coverage_of(o)
+        return res
 
     def _trace_from_cands(self, cands, n: int) -> List[Tuple[str, bytes]]:
         cap = n + 1
@@ -577,7 +623,9 @@ class ModelChecker:
             raise VsrError(rc, err.value.decode() or "no usable CUDA devices: the BFS has no CPU fallback")
         raw, sb = bytes(tr), self.state_bytes
         trace = [(ACTION_NAMES[acts[i]], raw[i * sb:(i + 1) * sb]) for i in range(int(st.trace_len))]
-        return self.result_from_stats(st, rc, trace)
+        res = self.result_from_stats(st, rc, trace)
+        res.coverage = self._coverage_of(o)
+        return res
 
     def simulate(self, num_walks: int = 1 << 20, depth: int = 100, seed: int = 1, device: int = 0, probe_walks: int = 0):
         """TLC's `-simulate -depth N`: random behaviours on the GPU.  Returns (VsrSimStats, trace) — the trace is the
@@ -648,6 +696,7 @@ class ModelChecker:
             res = self.result_from_stats(st, rc, trace, levels)
             res.liveness = live
             res.trace_loop = int(st.trace_loop)
+            res.coverage = self._coverage_of(o)
             return res
         finally:
             lib.vsr_engine_destroy(e)

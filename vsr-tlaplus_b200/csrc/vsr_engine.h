@@ -73,6 +73,9 @@ struct VsrEngine {
     double level_ms_insert_acc = 0; /* the part of level_ms_acc spent in launches that only insert records from peers */
     uint64_t records_sent = 0, records_received = 0;
     std::vector<std::vector<uint8_t>> collected; /* per level states (collect_levels) */
+    /* action coverage: this rank's counts per finished level and their sums; NULL = the run does not count (then the
+       kernels are launched without the counters: ExpandParams::cover stays NULL) */
+    VsrCoverage* cov = nullptr;
     /* liveness store (models with a property; vsr_live.cu): the not-P states of every finished level, grouped by level */
     uint32_t* live_words = nullptr;      /* [0, live_dev_cap) in HBM */
     uint32_t* live_words_host = nullptr; /* the rest in pinned host memory mapped into the device */
@@ -89,6 +92,8 @@ struct VsrEngine {
 
 int engine_reset_level(VsrEngine* e);
 void fill_params(VsrEngine* e, vsr::ExpandParams& p);
+/* turn the coverage counters on (cleared) or off; between runs only */
+void engine_set_coverage(VsrEngine* e, bool on);
 /* vsr_live.cu: the liveness store's allocation (after the BFS's, from what memory is left), release, clearing, and the
    per-level collection vsr_engine_finish_level calls for a model with a property */
 int live_create(VsrEngine* e, char* err, size_t errcap);

@@ -32,7 +32,7 @@ const GpuOps* find_gpu_ops(int R, int V, int K) {
 using namespace vsr;
 
 int engine_reset_level(VsrEngine* e) {
-    CK(cudaMemsetAsync(e->ctr, 0, sizeof(DevCounters), e->stream));
+    CK(cudaMemsetAsync(e->ctr, 0, e->cov ? sizeof(LevelCounters) : sizeof(DevCounters), e->stream));
     static const unsigned long long ones = ~0ull;
     CK(cudaMemcpyAsync(&e->ctr->viol_id, &ones, 8, cudaMemcpyHostToDevice, e->stream));
     CK(cudaMemcpyAsync(&e->ctr->dead_id, &ones, 8, cudaMemcpyHostToDevice, e->stream));
@@ -70,6 +70,17 @@ void fill_params(VsrEngine* e, ExpandParams& p) {
     p.world = e->world;
     p.owner_shift = e->owner_shift;
     p.push_cap = e->inbox_cap;
+    p.cover = e->cov ? reinterpret_cast<LevelCounters*>(e->ctr)->cover : nullptr;
+}
+
+void engine_set_coverage(VsrEngine* e, bool on) {
+    if (!on) {
+        delete e->cov;
+        e->cov = nullptr;
+        return;
+    }
+    if (!e->cov) e->cov = new VsrCoverage;
+    memset(e->cov, 0, sizeof *e->cov);
 }
 
 /* One launch of the wavefront kernel over p.n_in frontier states and p.drain_total records to insert: clears the
@@ -140,6 +151,7 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     e->owner_shift = world > 1 ? 64 - lg : 64;
     e->device = opts->device;
     memset(&e->st, 0, sizeof e->st);
+    engine_set_coverage(e, opts->coverage != nullptr);
     auto bail = [&](const char* what, cudaError_t c) {
         std::string msg = std::string(what) + ": " + cudaGetErrorString(c);
         vsr_engine_destroy(e);
@@ -189,7 +201,7 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
                 return bail("cudaHostAlloc(frontier spill)", ce);
     }
     if (e->trace_cap && (ce = cudaMallocAsync((void**)&e->trace, e->trace_cap * 8, e->stream)) != cudaSuccess) return bail("cudaMalloc(trace)", ce);
-    if ((ce = cudaMallocAsync((void**)&e->ctr, sizeof(DevCounters), e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
+    if ((ce = cudaMallocAsync((void**)&e->ctr, sizeof(LevelCounters), e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->ties, e->tie_cap * (size_t)e->g->tie_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->fp_tab, 8 * 256 * 8, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->init_rec, e->g->rec_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
@@ -225,6 +237,7 @@ void vsr_engine_destroy(VsrEngine* e) {
     if (e->stream) cudaFreeAsync(e->init_rec, e->stream); else cudaFree(e->init_rec);
     live_destroy(e);
     vsr_engine_detach(e);
+    delete e->cov;
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->stream) { cudaStreamSynchronize(e->stream); cudaStreamDestroy(e->stream); }
@@ -338,9 +351,11 @@ int vsr_engine_insert_records(VsrEngine* e, const void* dev_records, uint64_t n)
 }
 
 int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
-    DevCounters c;
-    CK(cudaMemcpyAsync(&c, e->ctr, sizeof c, cudaMemcpyDeviceToHost, e->stream));
-    e->st.bytes_d2h += sizeof c;
+    LevelCounters lc; /* with coverage the same copy reads the action counters behind DevCounters */
+    DevCounters& c = lc.c;
+    const size_t ctr_bytes = e->cov ? sizeof lc : sizeof c;
+    CK(cudaMemcpyAsync(&lc, e->ctr, ctr_bytes, cudaMemcpyDeviceToHost, e->stream));
+    e->st.bytes_d2h += ctr_bytes;
     CK(cudaStreamSynchronize(e->stream));
     const uint64_t fcap_total = e->frontier_cap + e->frontier_host_cap;
     if (c.tie_count > 0 && c.tie_count <= e->tie_cap && !c.overflow && c.out_count <= fcap_total) {
@@ -379,9 +394,9 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
         fill_params(e, p);
         CK(e->g->launch_patch(p, e->ties, nbest, c.out_count, e->stream));
         e->st.kernel_launches++;
-        CK(cudaMemcpyAsync(&c, e->ctr, sizeof c, cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaMemcpyAsync(&lc, e->ctr, ctr_bytes, cudaMemcpyDeviceToHost, e->stream));
         CK(cudaStreamSynchronize(e->stream));
-        e->st.bytes_d2h += host.size() + sizeof c;
+        e->st.bytes_d2h += host.size() + ctr_bytes;
         e->st.bytes_h2d += best.size();
     }
     VsrLevelInfo li;
@@ -437,6 +452,18 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
     if (n_new > 0 && gen_level - 1 < VSR_MAX_LEVELS) {
         e->st.level_sizes[gen_level - 1] = n_new;
         e->st.num_levels = gen_level;
+    }
+    if (e->cov && gen_level - 1 < VSR_MAX_LEVELS) {
+        bool any = false;
+        for (int a = 0; a < VSR_NUM_ACTIONS; a++) {
+            const uint64_t g = lc.cover[a], d = lc.cover[VSR_NUM_ACTIONS + a];
+            e->cov->level_generated[gen_level - 1][a] = g;
+            e->cov->level_distinct[gen_level - 1][a] = d;
+            e->cov->generated[a] += g;
+            e->cov->distinct[a] += d;
+            any |= g != 0;
+        }
+        if (any) e->cov->num_levels = gen_level;
     }
     if (li.violation && e->st.violation_level == 0) {
         e->st.violation_level = gen_level;
@@ -551,6 +578,7 @@ int vsr_engine_reset(VsrEngine* e) {
     e->cur = 0; e->n_cur = 0; e->cur_base = 0; e->next_base = 0; e->level = 0; e->level_open = false;
     e->records_sent = e->records_received = 0;
     e->collected.clear();
+    if (e->cov) memset(e->cov, 0, sizeof *e->cov);
     return live_reset(e);
 }
 
@@ -560,6 +588,18 @@ int vsr_engine_stats(const VsrEngine* e, VsrStats* out) {
 }
 
 const char* vsr_engine_last_error(const VsrEngine* e) { return e->last_error; }
+
+int vsr_engine_coverage(const VsrEngine* e, VsrCoverage* out) {
+    if (!e->cov) return VSR_RC_CONFIG_ERROR;
+    *out = *e->cov;
+    return 0;
+}
+
+size_t vsr_sizeof(const char* struct_name) {
+    const std::string n = struct_name ? struct_name : "";
+    return n == "VsrRunOpts" ? sizeof(VsrRunOpts) : n == "VsrCoverage" ? sizeof(VsrCoverage) : n == "VsrStats" ? sizeof(VsrStats)
+         : n == "VsrLevelInfo" ? sizeof(VsrLevelInfo) : 0;
+}
 
 /* number of states collected for `level` (1-based) and a copy of them (tests) */
 uint64_t vsr_engine_collected(const VsrEngine* e, int level, void* host_out, uint64_t cap_states) {

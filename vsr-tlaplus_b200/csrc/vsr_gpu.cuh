@@ -28,6 +28,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/vsr_flat.h" /* VSR_ACT_*, VSR_NUM_ACTIONS */
 #include "vsr_actions.h"
 
 namespace vsr {
@@ -52,6 +53,11 @@ struct DevCounters {
 #ifdef VSR_EXP_ROUNDCLK
     unsigned long long roundclk[5]; /* warp-cycles of this launch by phase (CLK_*); printed per level by the host */
 #endif
+};
+/* the engine's counter block: the coverage counters follow DevCounters, so that one memset clears and one copy reads both */
+struct LevelCounters {
+    DevCounters c;
+    unsigned long long cover[2 * VSR_NUM_ACTIONS]; /* ExpandParams::cover */
 };
 #ifdef VSR_EXP_ROUNDCLK
 /* phases of an expand warp's time: waiting at the end-of-round barrier, waiting at the scan's barriers (parents loaded,
@@ -112,6 +118,9 @@ struct ExpandParams {
     const uint8_t* drain[MAX_WORLD];
     unsigned int drain_n[MAX_WORLD];
     unsigned long long drain_total;
+    /* action coverage (the COVER instantiation only; NULL otherwise): [2][VSR_NUM_ACTIONS] counters of the level being
+       generated, by the action of the inserted record's candidate: sum of mult ("states generated"), then first arrivals */
+    unsigned long long* cover;
 };
 
 /* ------------------------------------------------------------------ primitives */
@@ -339,7 +348,9 @@ template <class L> struct ExpandCfg {
 /* MULTI: the instantiation for several GPUs (push_records in emit, drain after the rounds), and for every launch that inserts
    records (Init, vsr_engine_insert_records).  The one-GPU expansion has none of that code: it costs the hot path registers
    (380 vs 140 bytes of spills in emit at the 64-register budget). */
-template <class L, bool MULTI> struct Expander {
+/* COVER: the instantiation that also counts, per action of Next, what commit inserts (TLC's -coverage).  A run without
+   coverage launches the instantiations without it: the same code as before the counters existed. */
+template <class L, bool MULTI, bool COVER = false> struct Expander {
     typedef Ops<L> O_;
     typedef typename ExpandCfg<L>::Smem Smem;
     typedef typename Smem::Stage Stage;
@@ -478,6 +489,41 @@ template <class L, bool MULTI> struct Expander {
         }
     }
 
+    /* ---- action coverage (COVER).  Counted where a state is inserted, so local successors, records drained from peers,
+       Init and injected records are all counted once, at the owner (as `generated` is).  Per batch the warp aggregates by
+       action — a batch of the pool holds one group, i.e. one or two actions; a drained chunk may hold more — and its first
+       lane of each action adds the two sums to the block's table, which finish() adds to P.cover once per block.  The
+       table is 320 bytes of static shared memory where the layout's block leaves them (cover_budget), else P.cover itself. */
+    static constexpr int NCOV = 2 * VSR_NUM_ACTIONS;
+    static constexpr size_t SMEM_SPARE = 512; /* static shared memory beside Smem: the round counter and the table */
+    static_assert(NCOV * sizeof(unsigned long long) + sizeof(unsigned long long) <= SMEM_SPARE, "the table does not fit what ExpandCfg leaves beside Smem");
+    static constexpr bool COVER_SHARED = sizeof(Smem) + SMEM_SPARE <= (ExpandCfg<L>::BLOCKS == 1 ? 227 * 1024 : 113 * 1024);
+    static __device__ __forceinline__ unsigned long long* cover_table(const ExpandParams& P) {
+        if constexpr (COVER_SHARED) {
+            __shared__ unsigned long long tab[NCOV];
+            return tab;
+        } else {
+            return P.cover;
+        }
+    }
+    static __device__ __forceinline__ void cover_count(const ExpandParams& P, int lane, bool live, unsigned newmask, unsigned long long trec, unsigned gen) {
+        const int a = !live ? -1 : (trec >> 12) == ROOT_GID ? (int)VSR_ACT_INIT : O_::action_of((int)(trec & 0xFFFu));
+        unsigned long long* tab = cover_table(P);
+        unsigned todo = __ballot_sync(0xffffffffu, a >= 0);
+        while (todo) { /* warp-uniform: one turn per action present */
+            const int first = __ffs(todo) - 1;
+            const int act = __shfl_sync(0xffffffffu, a, first);
+            const unsigned m = __ballot_sync(0xffffffffu, a == act);
+            const unsigned g = __reduce_add_sync(0xffffffffu, a == act ? gen : 0u);
+            if (lane == first) {
+                atomicAdd(&tab[act], (unsigned long long)g);
+                const int n = __popc(m & newmask);
+                if (n) atomicAdd(&tab[VSR_NUM_ACTIONS + act], (unsigned long long)n);
+            }
+            todo &= ~m;
+        }
+    }
+
     /* the seen-set insert of one state per lane and everything after it — tie list, inline invariant, compaction of the
        survivors into the warp's staging area, flush — shared by the expansion (emit) and by the records of the drain
        (received from peers, Init, injected records): the only insert of a state in the library.  Returns this lane's
@@ -514,6 +560,7 @@ template <class L, bool MULTI> struct Expander {
         /* compaction of the survivors into the warp's staging area (one ballot, all lanes).  The survivors' final rows
            may overlap other lanes' scratch rows: every lane has read its row before anybody writes */
         const unsigned newmask = __ballot_sync(0xffffffffu, isnew);
+        if constexpr (COVER) cover_count(P, lane, live, newmask, trec, gen);
         __syncwarp();
         if (isnew) {
             const int slot = sn + __popc(newmask & ((1u << lane) - 1u));
@@ -885,17 +932,25 @@ template <class L, bool MULTI> struct Expander {
             atomicAdd(&P.ctr->generated, acc_gen);
             atomicAdd(&P.ctr->probes, acc_probes);
         }
+        if constexpr (COVER && COVER_SHARED) {
+            __syncthreads(); /* every warp's last batch is counted */
+            const unsigned long long* tab = cover_table(P);
+            if (tid < NCOV && tab[tid]) atomicAdd(&P.cover[tid], tab[tid]);
+        }
     }
 };
 
-template <class L, bool MULTI> __global__ void __launch_bounds__(ExpandCfg<L>::WARPS * 32, ExpandCfg<L>::BLOCKS) expand_kernel(const __grid_constant__ ExpandParams P) {
+template <class L, bool MULTI, bool COVER = false> __global__ void __launch_bounds__(ExpandCfg<L>::WARPS * 32, ExpandCfg<L>::BLOCKS) expand_kernel(const __grid_constant__ ExpandParams P) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     typedef typename ExpandCfg<L>::Smem Smem;
     Smem& B = *reinterpret_cast<Smem*>(smem_raw);
     for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) B.fp_tab[i] = P.fp_tab[i];
     __shared__ unsigned long long next_round;
-    Expander<L, MULTI> X(P, B);
+    Expander<L, MULTI, COVER> X(P, B);
     if ((threadIdx.x & 31) == 0) B.w[threadIdx.x >> 5].sn = 0;
+    if constexpr (COVER && Expander<L, MULTI, COVER>::COVER_SHARED) { /* cleared before the loop's first barrier */
+        if (threadIdx.x < Expander<L, MULTI, COVER>::NCOV) Expander<L, MULTI, COVER>::cover_table(P)[threadIdx.x] = 0;
+    }
     const unsigned long long nrounds = (P.n_in + Smem::NR - 1) / Smem::NR;
     if (threadIdx.x == 0) next_round = atomicAdd(&P.ctr->work_next, 1ull);
     VSR_CLK(X, OTHER);
@@ -951,7 +1006,18 @@ template <class L> __global__ void patch_ties_kernel(const ExpandParams P, const
         if (t->auxkey < Ops<L>::aux_key(w)) {
             const uint32_t* tw = (const uint32_t*)((const uint8_t*)t + sizeof(TieRec));
             for (int j = 0; j < L::NW; j++) { w[j] = tw[j]; st[j] = tw[j]; }
-            if (P.trace && P.out_base + i < P.trace_cap) P.trace[P.out_base + i] = make_trec(t->parent, t->cand);
+            if (P.trace && P.out_base + i < P.trace_cap) {
+                if (P.cover) { /* coverage follows the trace: the state now counts as found by the winner's action */
+                    const uint64_t was = P.trace[P.out_base + i];
+                    const int a0 = (was >> 12) == ROOT_GID ? (int)VSR_ACT_INIT : Ops<L>::action_of((int)(was & 0xFFFu));
+                    const int a1 = t->parent == ROOT_GID ? (int)VSR_ACT_INIT : Ops<L>::action_of((int)(t->cand & 0xFFFu));
+                    if (a0 != a1) {
+                        atomicAdd(&P.cover[VSR_NUM_ACTIONS + a0], ~0ull); /* - 1 */
+                        atomicAdd(&P.cover[VSR_NUM_ACTIONS + a1], 1ull);
+                    }
+                }
+                P.trace[P.out_base + i] = make_trec(t->parent, t->cand);
+            }
         }
     }
     const int bad = Ops<L>::invariant(P.run, w);

@@ -39,6 +39,7 @@ template <class L> struct GpuThunks {
     static cudaError_t prepare(int* blocks_per_sm) {
         cudaError_t e = cudaFuncSetAttribute(expand_kernel<L, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(typename ExpandCfg<L>::Smem));
         if (e == cudaSuccess) e = cudaFuncSetAttribute(expand_kernel<L, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(typename ExpandCfg<L>::Smem));
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(expand_kernel<L, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(typename ExpandCfg<L>::Smem));
         if (e != cudaSuccess) return e;
         int a = 0, b = 0;
         e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, expand_kernel<L, false>, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem));
@@ -47,8 +48,11 @@ template <class L> struct GpuThunks {
         return e;
     }
     static cudaError_t launch_expand(const ExpandParams& p, int grid, cudaStream_t st) {
-        /* the one-GPU instantiation has no drain: records to insert (drain_total) need the MULTI one at any world size */
-        if (p.world > 1 || p.drain_total) expand_kernel<L, true><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
+        /* the one-GPU instantiation has no drain: records to insert (drain_total) need the MULTI one at any world size.
+           Coverage has one instantiation per layout, the MULTI one, for every launch of a run that counts (one more kernel
+           to compile per layout, not two); the grid and the block are the same for all three */
+        if (p.cover) expand_kernel<L, true, true><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
+        else if (p.world > 1 || p.drain_total) expand_kernel<L, true><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
         else expand_kernel<L, false><<<grid, ExpandCfg<L>::WARPS * 32, sizeof(typename ExpandCfg<L>::Smem), st>>>(p);
         return cudaGetLastError();
     }

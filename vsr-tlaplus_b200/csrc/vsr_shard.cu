@@ -238,6 +238,13 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     if (trace_len) *trace_len = 0;
     VsrGroup* g = e->group;
     if (e->world > 1 && (!g || !e->inbox || e->stage)) return set_error(e, "vsr_bfs_sharded needs vsr_engine_attach_group first");
+    if (opts->coverage && (opts->checkpoint_path || opts->recover_path)) {
+        snprintf(e->last_error, sizeof e->last_error, "coverage with -checkpoint / -recover: the coverage counters are not part of a checkpoint");
+        return VSR_RC_CONFIG_ERROR;
+    }
+    engine_set_coverage(e, opts->coverage != nullptr);
+    std::vector<VsrCoverage> cov(opts->coverage ? 1 : 0); /* the job's totals (the engine's own are this rank's) */
+    if (opts->coverage) memset(&cov[0], 0, sizeof cov[0]);
     if (e->m->info.property && (opts->checkpoint_path || opts->recover_path)) {
         snprintf(e->last_error, sizeof e->last_error, "-checkpoint / -recover with PROPERTY ViewChangeCompletes: checkpointing the liveness store is not supported");
         return VSR_RC_CONFIG_ERROR;
@@ -318,6 +325,29 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
             ms = std::max(ms, all[r].ms); msi = std::max(msi, all[r].ms_insert);
         }
         if (failed) { rc = failed; break; }
+        if (opts->coverage && level - 1 < VSR_MAX_LEVELS) { /* the level's action counts, summed over the ranks */
+            uint64_t sum[2][VSR_NUM_ACTIONS], parts[MAX_WORLD][VSR_NUM_ACTIONS];
+            static_assert(sizeof parts[0] <= VSR_GROUP_MSG_BYTES, "one all-gather per vector");
+            for (int k = 0; k < 2; k++) {
+                const uint64_t* row = k ? e->cov->level_distinct[level - 1] : e->cov->level_generated[level - 1];
+                memcpy(sum[k], row, sizeof sum[k]);
+                if (W > 1) {
+                    if (vsr_group_allgather(g, row, sizeof parts[0], parts)) return set_error(e, "%s", g->last_error);
+                    memset(sum[k], 0, sizeof sum[k]);
+                    for (int r = 0; r < W; r++)
+                        for (int a = 0; a < VSR_NUM_ACTIONS; a++) sum[k][a] += parts[r][a];
+                }
+            }
+            bool any = false;
+            for (int a = 0; a < VSR_NUM_ACTIONS; a++) {
+                cov[0].level_generated[level - 1][a] = sum[0][a];
+                cov[0].level_distinct[level - 1][a] = sum[1][a];
+                cov[0].generated[a] += sum[0][a];
+                cov[0].distinct[a] += sum[1][a];
+                any |= sum[0][a] != 0;
+            }
+            if (any) cov[0].num_levels = level;
+        }
         kernel_ms += ms;
         insert_ms += msi;
         tot.generated += n_gen;
@@ -466,6 +496,7 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     tot.seconds_insert = insert_ms * 1e-3;
     tot.seconds_total = now_s() - t0;
     *stats = tot;
+    if (opts->coverage) *opts->coverage = cov[0];
     return result;
 }
 
@@ -492,11 +523,13 @@ int vsr_bfs_multi(const VsrModel* m, const VsrRunOpts* opts, int ngpus, uint64_t
     std::vector<int> rcs(ngpus, 0), lens(ngpus, 0);
     std::vector<std::vector<uint32_t>> cands(ngpus, std::vector<uint32_t>(4096));
     std::vector<std::string> errors(ngpus);
+    std::vector<VsrCoverage> covs(opts->coverage ? ngpus : 0); /* every rank writes the same totals: rank 0's go to the caller */
     std::vector<std::thread> threads;
     for (int r = 0; r < ngpus; r++) {
         threads.emplace_back([&, r]() {
             VsrRunOpts o = *opts;
             o.device = opts->device + (one_device ? 0 : r);
+            if (opts->coverage && r > 0) o.coverage = &covs[r];
             char msg[256] = {0};
             VsrEngine* e = nullptr;
             int rc = vsr_engine_create(m, &o, r, ngpus, &e, msg, sizeof msg);

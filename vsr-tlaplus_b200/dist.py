@@ -116,6 +116,7 @@ class ShardedResult:
     bytes_d2h: int = 0
     trace_cands: List[int] = field(default_factory=list)
     trace: List[Tuple[str, bytes]] = field(default_factory=list)
+    coverage: Optional["ck.Coverage"] = None  # GpuEngine(coverage=True): the job's action coverage (the same on every rank)
     # check_sharded only: this rank's wall clock of the one-call API by part (engine creation = allocation + clearing the
     # seen-set; attach = inbox allocation + CUDA IPC mapping of the peers; bfs; replay of the counterexample; teardown)
     call_seconds: dict = field(default_factory=dict)
@@ -126,14 +127,18 @@ class GpuEngine:
 
     def __init__(self, mc: "ck.ModelChecker", rank: int, world: int, device: int = 0, table_capacity: int = 0,
                  frontier_capacity: int = 0, inbox_records: int = 0, keep_trace: bool = True, check_deadlock: bool = False,
-                 collect_levels: bool = False, group: Optional[Group] = None, exchange: str = "p2p", frontier_host_capacity: int = 0):
+                 collect_levels: bool = False, group: Optional[Group] = None, exchange: str = "p2p", frontier_host_capacity: int = 0,
+                 coverage: bool = False):
+        if coverage and world > 1 and exchange != "p2p":
+            # the staged pump (ShardedBfs) sums no per-level action counts over the ranks
+            raise ck.VsrError(151, "coverage with exchange='staged' is not supported: use the fused exchange (exchange='p2p')")
         self.mc, self.rank, self.world = mc, rank, world
         self.lib = mc._lib
         self.dev = torch.device("cuda", device)
         self.exchange = exchange if world > 1 else "none"
         self._opts = mc.run_opts(deadlock=check_deadlock, device=device, table_capacity=table_capacity,
                                  frontier_capacity=frontier_capacity, keep_trace=keep_trace, collect_levels=collect_levels,
-                                 frontier_host_capacity=frontier_host_capacity)
+                                 frontier_host_capacity=frontier_host_capacity, coverage=coverage)
         self._e = C.c_void_p()
         err = C.create_string_buffer(512)
         t0 = time.time()
@@ -196,6 +201,7 @@ class GpuEngine:
                           launches=int(st.kernel_launches), bytes_h2d=int(st.bytes_h2d), bytes_d2h=int(st.bytes_d2h))
         if want_trace and (rc in (11, 12) or r.violation_level):
             r.trace_cands = [int(cands[i]) for i in range(int(n.value))]
+        r.coverage = self.mc._coverage_of(o)
         return r
 
     # -- the stepwise interface (staged pump, tests) ----------------------------------------------------
@@ -244,6 +250,12 @@ class GpuEngine:
         self.lib.vsr_engine_stats(self._e, C.byref(st))
         return st
 
+    def coverage(self) -> "ck.Coverage":
+        """THIS rank's action coverage of the levels finished so far (an engine created with coverage=True)"""
+        cov = ck.VsrCoverage()
+        self._ck(self.lib.vsr_engine_coverage(self._e, C.byref(cov)))
+        return ck.Coverage.from_struct(cov)
+
     def trace_record(self, local_id: int) -> Tuple[int, int]:
         parent, cand = C.c_uint64(), C.c_uint32()
         self._ck(self.lib.vsr_engine_trace_record(self._e, local_id, C.byref(parent), C.byref(cand)))
@@ -282,10 +294,11 @@ class GpuEngine:
 
 def check_sharded(mc: "ck.ModelChecker", group: Group, device: int = 0, table_capacity: int = 0, frontier_capacity: int = 0,
                   inbox_records: int = 0, part_states: int = 0, keep_trace: bool = True, check_deadlock: bool = False,
-                  **run_kw) -> ShardedResult:
-    """One call per rank: engine + inbox + BFS + teardown; on a violation rank 0's result carries the literal trace."""
+                  coverage: bool = False, **run_kw) -> ShardedResult:
+    """One call per rank: engine + inbox + BFS + teardown; on a violation rank 0's result carries the literal trace.
+    coverage: count TLC's action coverage (ShardedResult.coverage, the job's totals on every rank)."""
     eng = GpuEngine(mc, group.rank, group.world, device=device, table_capacity=table_capacity, frontier_capacity=frontier_capacity,
-                    inbox_records=inbox_records, keep_trace=keep_trace, check_deadlock=check_deadlock, group=group)
+                    inbox_records=inbox_records, keep_trace=keep_trace, check_deadlock=check_deadlock, group=group, coverage=coverage)
     res = None
     try:
         t0 = time.time()
