@@ -147,7 +147,9 @@ typedef struct VsrRunOpts {
        states/ metadir, i.e. its users run with checkpoints).  checkpoint_path: file written at the first level boundary after
        checkpoint_seconds since the last one (0 = after every level; written to <path>.tmp and renamed, so an interrupted write
        leaves the previous checkpoint intact); recover_path: continue the BFS from that file instead of Init.  With several
-       ranks every rank uses <path>.rank<r>.  NULL = off. */
+       ranks every rank uses <path>.rank<r>.  A checkpoint written by another number of ranks (<path> of one rank, or
+       <path>.rank0 ... of several) is recovered too: every rank reads every old file and keeps the seen-set entries,
+       frontier states and trace records it owns.  NULL = off. */
     const char* checkpoint_path;
     const char* recover_path;
     double checkpoint_seconds;
@@ -242,7 +244,8 @@ int vsr_engine_stats(const VsrEngine* e, VsrStats* out);
 int vsr_engine_lookup(VsrEngine* e, const void* state, int* level_out, int* owner_out);
 /* Checkpoint of this rank's shard at a level boundary (after vsr_engine_finish_level, before the next expansion): the
  * current frontier, every seen-set entry {fingerprint, meta}, the trace records and the run's statistics, to one file.
- * vsr_engine_recover loads it into a fresh (or reset) engine of the same model, rank and world; the seen-set is re-inserted
+ * vsr_engine_recover loads it into a fresh (or reset) engine of the same model, rank and world (the primitive for one
+ * rank's own file; vsr_bfs_sharded also re-shards a checkpoint of another world); the seen-set is re-inserted
  * entry by entry, so its capacity may differ from the one the checkpoint was written with.  `totals` (may be NULL) travels
  * with the file: vsr_bfs_sharded stores the job's running totals there.  150 = not a checkpoint of this model. */
 int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals);
@@ -335,13 +338,14 @@ int vsr_engine_attach_staged(VsrEngine* e, uint64_t inbox_records, void** stage_
 int vsr_engine_detach(VsrEngine* e);                                 /* collective when attached to a group */
 uint64_t vsr_engine_default_inbox_records(const VsrEngine* e);
 /* The whole BFS, called by every rank of the group with the same opts (world 1: one call, no group); it starts from Init,
- * or from opts.recover_path, whatever the engine explored before.  All ranks return the same rc and the same totals
+ * or from opts.recover_path — a checkpoint of any world (1, 2, 4 or 8 ranks) — whatever the engine explored before.  All ranks return the same rc and the same totals
  * (records_sent / received, bytes_* and kernel_launches are this rank's).  part_states = frontier states per rank and step
  * (0 = from the inbox size).  On a violation / deadlock trace_cands[0 .. *trace_len) is the candidate chain from Init,
  * walked across ranks: vsr_replay_candidates turns it into the literal behaviour. */
 int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, VsrStats* stats, uint32_t* trace_cands, int* trace_len,
                     size_t trace_cap);
-/* `vsrmc -gpus N`: the same from ONE process, one thread per GPU (devices opts->device ... + ngpus - 1) */
+/* `vsrmc -gpus N`: the same from ONE process, one thread per GPU (devices opts->device ... + ngpus - 1); opts.recover_path
+ * may have been written by any number of GPUs */
 int vsr_bfs_multi(const VsrModel* m, const VsrRunOpts* opts, int ngpus, uint64_t inbox_records, uint64_t part_states, VsrStats* stats,
                   void* trace_out, uint8_t* trace_actions, size_t trace_cap, char* err, size_t errcap);
 

@@ -536,7 +536,8 @@ class ModelChecker:
                  frontier_host_capacity: int = 0, checkpoint_path: Optional[str] = None, recover_path: Optional[str] = None,
                  checkpoint_seconds: float = 0.0, coverage: bool = False) -> VsrRunOpts:
         """checkpoint_path / recover_path / checkpoint_seconds: TLC's -checkpoint / -recover (a file per rank at level
-        boundaries; see include/vsr_b200.h VsrRunOpts).  coverage: count TLC's action coverage (CheckResult.coverage)"""
+        boundaries; see include/vsr_b200.h VsrRunOpts).  recover_path may have been written by any number of GPUs: check()
+        and check_multi() re-shard it as they load it.  coverage: count TLC's action coverage (CheckResult.coverage)"""
         o = VsrRunOpts()
         if coverage:
             o.cov = VsrCoverage()  # kept alive by the options object
@@ -611,7 +612,8 @@ class ModelChecker:
         return [(ACTION_NAMES[acts[i]], raw[i * sb:(i + 1) * sb]) for i in range(m)]
 
     def check_multi(self, gpus: int, inbox_records: int = 0, part_states: int = 0, **kw) -> CheckResult:
-        """The BFS sharded over `gpus` GPUs from THIS process (one thread per GPU): ``vsr_bfs_multi``, what `vsrmc -gpus N` runs."""
+        """The BFS sharded over `gpus` GPUs from THIS process (one thread per GPU): ``vsr_bfs_multi``, what `vsrmc -gpus N` runs.
+        recover_path= continues a checkpoint written by any number of GPUs."""
         o = self.run_opts(**kw)
         st = VsrStats()
         cap = 512

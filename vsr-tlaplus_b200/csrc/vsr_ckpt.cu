@@ -69,15 +69,25 @@ __global__ void ckpt_compact_kernel(const uint64_t* __restrict__ table, unsigned
     }
 }
 
-/* entries of a checkpoint back into a (fresh) table: every one must be new */
+/* entries of a checkpoint back into a (fresh) table: every one must be new.  owner_shift < 64 (a checkpoint of another
+   number of ranks): only the entries this rank owns, counted in *owned; 64 inserts every entry */
 __global__ void ckpt_reinsert_kernel(uint64_t* table, unsigned long long cap, const uint64_t* __restrict__ ents, unsigned long long n,
-                                     unsigned long long* not_new) {
-    unsigned long long bad = 0;
+                                     int owner_shift, int rank, unsigned long long* not_new, unsigned long long* owned) {
+    unsigned long long bad = 0, mine = 0;
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        if (owner_shift < 64 && owner_of(ents[2 * i], owner_shift) != rank) continue;
         unsigned probes = 0, coll = 0;
+        mine++;
         if (table_insert(table, cap, ents[2 * i], ents[2 * i + 1], probes, coll) != INS_NEW) bad++;
     }
     if (bad) atomicAdd(not_new, bad);
+    if (owned && mine) atomicAdd(owned, mine);
+}
+
+/* old trace records renumbered into the new world's ids */
+__global__ void ckpt_remap_trace_kernel(const uint64_t* __restrict__ in, unsigned long long n, uint64_t* __restrict__ out, const GidRemap m) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
+        out[i] = remap_trec(m, in[i]);
 }
 
 struct File {
@@ -107,6 +117,28 @@ int frontier_from_host(VsrEngine* e, int buf, uint64_t first, uint64_t n, const 
 }
 
 constexpr uint64_t IO_CHUNK = 64ull << 20; /* bytes per host staging round */
+
+bool header_ok(const CkptHeader& h) {
+    return h.magic == CKPT_MAGIC && h.version == 1 && h.header_bytes == sizeof h && h.stats_bytes == sizeof(VsrStats);
+}
+
+/* 1: a checkpoint header of this build, 0: something else, -1: the file cannot be opened */
+int peek_header(const std::string& path, CkptHeader& h) {
+    File in;
+    in.f = fopen(path.c_str(), "rb");
+    if (!in.f) return -1;
+    return fread(&h, sizeof h, 1, in.f) == 1 && header_ok(h) ? 1 : 0;
+}
+
+/* file offsets of a checkpoint's sections */
+constexpr uint64_t SECTIONS = sizeof(CkptHeader) + 2 * sizeof(VsrStats);
+uint64_t entries_at(const CkptHeader& h) { return SECTIONS + h.n_cur * h.state_bytes; }
+uint64_t trace_at(const CkptHeader& h) { return entries_at(h) + h.n_entries * 16; }
+
+int seek(VsrEngine* e, File& f, uint64_t at, const char* path) {
+    if (fseeko(f.f, (off_t)at, SEEK_SET) != 0) return io_error(e, "truncated", path);
+    return 0;
+}
 
 } // namespace
 
@@ -267,7 +299,7 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
             const uint64_t k = std::min(per, h.n_entries - o);
             if (fread(host.data(), 16, k, in.f) != k) return io_error(e, "truncated", path);
             CK(cudaMemcpyAsync(scratch, host.data(), k * 16, cudaMemcpyHostToDevice, e->stream));
-            ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, scratch, k, dbad);
+            ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, scratch, k, 64, 0, dbad, nullptr);
             CK(cudaGetLastError());
             CK(cudaStreamSynchronize(e->stream)); /* `host` is reused by the next round */
         }
@@ -303,3 +335,271 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
 }
 
 } /* extern "C" */
+
+/* ------------------------------------------------------------------ recovery on another number of ranks
+ * Ownership is a pure function of the fingerprint, so the old files already hold everything a new rank needs: every rank of
+ * the recovering world reads EVERY old file and keeps its own share — no exchange between the ranks, no peer memory.
+ *   seen-set  the entries it owns (ckpt_reinsert_kernel's owner filter)
+ *   frontier  the states it owns (reshard_frontier_kernel: the BFS's fingerprint and owner rule), appended to buffer 0, each
+ *             with a copy of its old trace record; every kept state must be in the seen-set just filled
+ *   trace     one global order of the old records, F(r, l) = off[r] + l, cut into W_new slices (GidRemap); the rank loads
+ *             its slice, renumbering every parent, and its frontier's records follow the slice
+ * A checkpoint of W_old ranks is read W_new times over in all.  The job's totals travel unchanged (the violation id renumbered);
+ * of this rank's own counters only `distinct` (= entries it inserted, which its next checkpoint checks) carries over: the
+ * per-rank work counters (generated, probes, launches, records sent / received, ...) start at 0. */
+
+int ckpt_old_files(VsrEngine* e, const char* base, std::vector<std::string>& files) {
+    files.clear();
+    const std::string P = base, P0 = P + ".rank0";
+    CkptHeader h1, h0;
+    const int k1 = peek_header(P, h1), k0 = peek_header(P0, h0);
+    const int W = e->world;
+    const int k = W > 1 ? k0 : k1;
+    const CkptHeader& h = W > 1 ? h0 : h1;
+    if (k == 0 || (k == 1 && h.world == W)) return 0; /* this world's own files (or not a checkpoint: vsr_engine_recover says so) */
+    const bool one = k1 == 1 && h1.world == 1;       /* what a one-rank writer leaves */
+    if (one && k0 == 1) {
+        snprintf(e->last_error, sizeof e->last_error, "recover: both %s (1 rank) and %s (%d ranks) exist and neither was written by %d ranks: remove one",
+                 P.c_str(), P0.c_str(), h0.world, W);
+        return VSR_RC_CONFIG_ERROR;
+    }
+    if (k0 == 1) {
+        if (h0.world < 1 || h0.world > MAX_WORLD) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s claims a world of %d ranks", P0.c_str(), h0.world);
+            return VSR_RC_SPEC_ERROR;
+        }
+        for (int r = 0; r < h0.world; r++) files.push_back(P + ".rank" + std::to_string(r));
+    } else if (one || k1 == 0) {
+        files.push_back(P); /* k1 == 0 (several ranks): not a checkpoint, which the loader reports by name */
+    } else if (k0 == 0) {
+        files.push_back(P0);
+    }
+    return 0; /* no file at all: vsr_engine_recover reports this world's missing file */
+}
+
+int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, VsrStats* totals_out) {
+    CK(cudaSetDevice(e->device));
+    const int Wold = (int)files.size(), W = e->world, me = e->rank;
+    const uint64_t S = (uint64_t)e->g->bytes;
+    const double t_start = now_s();
+    double t_read = 0, t_insert = 0, t_frontier = 0, t_trace = 0;
+    uint64_t bytes_read = 0;
+    std::vector<File> in(Wold);
+    std::vector<CkptHeader> h(Wold);
+    VsrStats tot, mine, other;
+    /* 1. every old file: a checkpoint of this model, rank r of Wold, of the same level and job */
+    for (int r = 0; r < Wold; r++) {
+        const char* path = files[r].c_str();
+        in[r].f = fopen(path, "rb");
+        if (!in[r].f) return io_error(e, "cannot open", path);
+        if (fread(&h[r], sizeof h[r], 1, in[r].f) != 1 || !header_ok(h[r])) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s is not a checkpoint of this build", path);
+            return VSR_RC_SPEC_ERROR;
+        }
+        if (fread(&mine, sizeof mine, 1, in[r].f) != 1 || fread(r ? &other : &tot, sizeof tot, 1, in[r].f) != 1) return io_error(e, "truncated", path);
+        const CkptHeader& x = h[r];
+        if (x.state_bytes != S || x.R != e->g->R || x.V != e->g->V || x.K != e->g->K || x.symmetry != e->m->run.symmetry || x.use_view != e->m->run.use_view ||
+            x.invariant != e->m->run.invariant) {
+            snprintf(e->last_error, sizeof e->last_error,
+                     "recover: %s was written for ReplicaCount=%d |Values|=%d StartViewOnTimerLimit=%d symmetry=%d view=%d invariants=%d: not this model", path,
+                     x.R, x.V, x.K - 1, x.symmetry, x.use_view, x.invariant);
+            return VSR_RC_SPEC_ERROR;
+        }
+        if (x.world != Wold || x.rank != r) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s is rank %d of %d, expected rank %d of %d", path, x.rank, x.world, r, Wold);
+            return VSR_RC_SPEC_ERROR;
+        }
+        if (r && (x.level != h[0].level || x.keep_trace != h[0].keep_trace || memcmp(&other, &tot, sizeof tot) != 0)) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s is not of the same checkpoint as %s (level, trace or job totals differ)", path, files[0].c_str());
+            return VSR_RC_SPEC_ERROR;
+        }
+        if (x.n_trace && x.n_trace != x.next_base) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s holds %llu of its %llu trace records", path, (unsigned long long)x.n_trace,
+                     (unsigned long long)x.next_base);
+            return VSR_RC_SPEC_ERROR;
+        }
+    }
+    /* 2. the id mapping: old records in file order, cut into W slices */
+    GidRemap m;
+    memset(&m, 0, sizeof m);
+    m.old_world = Wold;
+    uint64_t T = 0;
+    for (int r = 0; r < Wold; r++) {
+        m.off[r] = T;
+        T += h[r].next_base;
+    }
+    if (e->trace && !h[0].keep_trace && T) {
+        snprintf(e->last_error, sizeof e->last_error, "recover: %s was written without trace records; continue it with keep_trace off (vsrmc -notrace)", files[0].c_str());
+        return VSR_RC_CONFIG_ERROR;
+    }
+    m.slice = std::max<uint64_t>(1, (T + W - 1) / W);
+    const uint64_t lo = std::min<uint64_t>(T, (uint64_t)me * m.slice), hi = std::min<uint64_t>(T, lo + m.slice);
+    const uint64_t cur_base = hi - lo;
+    int rc = vsr_engine_reset(e);
+    if (rc) return rc;
+    e->touched = true; /* from here on a failure leaves part of the checkpoint in the engine */
+    CK(cudaStreamSynchronize(e->stream));
+    std::vector<uint8_t> host;
+    unsigned long long* d0 = &e->ctr->work_next; /* scratch words: the level's counters are reset when it opens */
+    unsigned long long* d1 = &e->ctr->drain_next;
+    uint8_t* scratch = (uint8_t*)e->frontier[1];
+    const uint64_t scratch_bytes = e->frontier_cap * S;
+    /* 3. the seen-set entries this rank owns.  Chunks of at most 1/16 of the table: the load is checked after every chunk,
+       so a share that does not fit stops at 15/16 load, where inserts still end */
+    const uint64_t limit = e->table_cap - e->table_cap / 8;
+    unsigned long long counts[2] = {0, 0}; /* entries not new, entries owned */
+    uint64_t n_entries = 0;
+    for (int r = 0; r < Wold; r++) n_entries += h[r].n_entries;
+    {
+        const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>({IO_CHUNK / 16, scratch_bytes / 16, e->table_cap / 16}));
+        CK(cudaMemsetAsync(d0, 0, 16, e->stream));
+        host.resize(per * 16);
+        for (int r = 0; r < Wold; r++) {
+            if ((rc = seek(e, in[r], entries_at(h[r]), files[r].c_str()))) return rc;
+            for (uint64_t o = 0; o < h[r].n_entries; o += per) {
+                const uint64_t k = std::min(per, h[r].n_entries - o);
+                double t = now_s();
+                if (fread(host.data(), 16, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                t_read += now_s() - t;
+                t = now_s();
+                CK(cudaMemcpyAsync(scratch, host.data(), k * 16, cudaMemcpyHostToDevice, e->stream));
+                ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, (const uint64_t*)scratch, k, e->owner_shift, me, d0, d1);
+                CK(cudaGetLastError());
+                CK(cudaMemcpyAsync(counts, d0, 16, cudaMemcpyDeviceToHost, e->stream));
+                CK(cudaStreamSynchronize(e->stream)); /* `host` is reused by the next round */
+                t_insert += now_s() - t;
+                bytes_read += k * 16;
+                e->st.bytes_h2d += k * 16;
+                if (counts[1] > limit) {
+                    snprintf(e->last_error, sizeof e->last_error,
+                             "capacity exceeded (recover): rank %d of %d owns more than %llu of the checkpoint's %llu seen-set entries: 7/8 of its %llu slots",
+                             me, W, (unsigned long long)limit, (unsigned long long)n_entries, (unsigned long long)e->table_cap);
+                    return VSR_RC_TOO_LARGE;
+                }
+            }
+        }
+        if (counts[0]) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %llu seen-set entries of %s and the other ranks' files could not be inserted as new (corrupt file?)", counts[0],
+                     files[0].c_str());
+            return VSR_RC_ERROR;
+        }
+    }
+    const uint64_t owned = counts[1];
+    /* 4. the frontier states this rank owns, into buffer 0, with their trace records after this rank's slice */
+    uint64_t kept = 0;
+    {
+        const uint64_t fcap_total = e->frontier_cap + e->frontier_host_cap;
+        const bool tr = e->trace && h[0].keep_trace;
+        const uint64_t per = std::max<uint64_t>(1, (std::min(IO_CHUNK, scratch_bytes) - 16) / (S + 8));
+        const uint64_t tr_off = (per * S + 15) & ~15ull;
+        ReshardParams q;
+        memset(&q, 0, sizeof q);
+        q.in = (const uint32_t*)scratch;
+        q.in_trace = tr ? (const uint64_t*)(scratch + tr_off) : nullptr;
+        q.out = e->frontier[0];
+        q.out_hi = e->frontier_host[0];
+        q.out_split = e->frontier_host_cap ? e->frontier_cap : ~0ull;
+        q.out_cap = fcap_total;
+        q.trace = tr ? e->trace : nullptr;
+        q.trace_base = cur_base;
+        q.trace_cap = e->trace_cap;
+        q.table = e->table;
+        q.table_cap = e->table_cap;
+        q.fp_tab = e->fp_tab;
+        q.run = e->m->run;
+        q.rank = me;
+        q.owner_shift = e->owner_shift;
+        q.level = h[0].level;
+        q.remap = m;
+        q.kept = d0;
+        q.missing = d1;
+        CK(cudaMemsetAsync(d0, 0, 16, e->stream));
+        host.resize(per * (S + 8));
+        uint64_t* host_tr = (uint64_t*)(host.data() + per * S);
+        for (int r = 0; r < Wold; r++) {
+            const uint64_t n_cur = h[r].n_cur;
+            for (uint64_t o = 0; o < n_cur; o += per) {
+                const uint64_t k = std::min(per, n_cur - o);
+                double t = now_s();
+                if ((rc = seek(e, in[r], SECTIONS + o * S, files[r].c_str()))) return rc;
+                if (fread(host.data(), S, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                if (tr) {
+                    if ((rc = seek(e, in[r], trace_at(h[r]) + (h[r].cur_base + o) * 8, files[r].c_str()))) return rc;
+                    if (fread(host_tr, 8, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                }
+                t_read += now_s() - t;
+                t = now_s();
+                CK(cudaMemcpyAsync(scratch, host.data(), k * S, cudaMemcpyHostToDevice, e->stream));
+                if (tr) CK(cudaMemcpyAsync(scratch + tr_off, host_tr, k * 8, cudaMemcpyHostToDevice, e->stream));
+                q.n = k;
+                CK(e->g->launch_reshard_frontier(q, e->sms, e->stream));
+                CK(cudaStreamSynchronize(e->stream));
+                e->st.kernel_launches++;
+                t_frontier += now_s() - t;
+                bytes_read += k * (S + (tr ? 8 : 0));
+                e->st.bytes_h2d += k * (S + (tr ? 8 : 0));
+            }
+        }
+        CK(cudaMemcpy(counts, d0, 16, cudaMemcpyDeviceToHost));
+        kept = counts[0];
+        if (kept > fcap_total) {
+            snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (recover): rank %d of %d owns %llu of the checkpoint's frontier states, its frontier holds %llu",
+                     me, W, (unsigned long long)kept, (unsigned long long)fcap_total);
+            return VSR_RC_TOO_LARGE;
+        }
+        if (counts[1]) {
+            snprintf(e->last_error, sizeof e->last_error,
+                     "recover: the checkpoint's frontier and seen-set disagree: %llu frontier states rank %d owns are not in its seen-set at depth %d", counts[1], me, h[0].level);
+            return VSR_RC_ERROR;
+        }
+        if (tr && cur_base + kept > e->trace_cap) {
+            snprintf(e->last_error, sizeof e->last_error,
+                     "capacity exceeded (recover): rank %d needs %llu trace records (%llu of the checkpoint's %llu, then %llu frontier copies), it holds %llu", me,
+                     (unsigned long long)(cur_base + kept), (unsigned long long)cur_base, (unsigned long long)T, (unsigned long long)kept, (unsigned long long)e->trace_cap);
+            return VSR_RC_TOO_LARGE;
+        }
+    }
+    /* 5. this rank's slice [lo, hi) of the old records, from whichever files hold it, renumbered on the device */
+    if (e->trace && h[0].keep_trace) {
+        const uint64_t per = std::max<uint64_t>(1, std::min(IO_CHUNK, scratch_bytes) / 8);
+        host.resize(per * 8);
+        for (int r = 0; r < Wold; r++) {
+            const uint64_t a = std::max<uint64_t>(lo, m.off[r]), b = std::min<uint64_t>(hi, m.off[r] + h[r].next_base);
+            if (a >= b) continue;
+            if ((rc = seek(e, in[r], trace_at(h[r]) + (a - m.off[r]) * 8, files[r].c_str()))) return rc;
+            for (uint64_t o = a; o < b; o += per) {
+                const uint64_t k = std::min(per, b - o);
+                double t = now_s();
+                if (fread(host.data(), 8, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                t_read += now_s() - t;
+                t = now_s();
+                CK(cudaMemcpyAsync(scratch, host.data(), k * 8, cudaMemcpyHostToDevice, e->stream));
+                ckpt_remap_trace_kernel<<<e->sms * 4, 256, 0, e->stream>>>((const uint64_t*)scratch, k, e->trace + (o - lo), m);
+                CK(cudaGetLastError());
+                CK(cudaStreamSynchronize(e->stream));
+                t_trace += now_s() - t;
+                bytes_read += k * 8;
+                e->st.bytes_h2d += k * 8;
+            }
+        }
+    }
+    /* the BFS position: the frontier of depth `level`, this rank's ids continue after its slice */
+    e->st.distinct = owned;
+    e->n_cur = kept;
+    e->cur_base = cur_base;
+    e->next_base = cur_base + kept;
+    e->cur = 0;
+    e->level = h[0].level;
+    e->level_open = false;
+    if (e->opts.collect_levels) e->collected.resize(h[0].level);
+    e->records_sent = e->records_received = 0;
+    if (tot.violation_level) tot.violation_id = remap_gid(m, tot.violation_id);
+    if (totals_out) *totals_out = tot;
+    if (e->opts.verbose)
+        fprintf(stderr,
+                "recover: rank %d of %d took its share of %d checkpoint files (%llu bytes read) in %.3f s: %.3f s reading, %.3f s seen-set insert, %.3f s frontier, %.3f s trace; "
+                "%llu seen-set entries, %llu frontier states\n",
+                me, W, Wold, (unsigned long long)bytes_read, now_s() - t_start, t_read, t_insert, t_frontier, t_trace, (unsigned long long)owned,
+                (unsigned long long)kept);
+    return 0;
+}

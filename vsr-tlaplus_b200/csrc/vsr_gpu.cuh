@@ -1097,6 +1097,81 @@ template <class L> __global__ void audit_frontier_kernel(const ExpandParams P, u
     audit_add(&out->words_xor, wx, true);
 }
 
+/* ------------------------------------------------------------------ re-sharding a checkpoint (vsr_ckpt.cu)
+   A checkpoint written by W_old ranks, continued by W_new ranks.  Every old trace record gets a place in one global order,
+   F(r, l) = off[r] + l (off = prefix sum of the old files' record counts), and the new world cuts that order into slices of
+   `slice` records: F lands on rank F / slice at local id F % slice.  Every stored global id (trace parents, the totals'
+   violation id) is renumbered with this one function, so the parent walk reads the new ids as it read the old ones. */
+struct GidRemap {
+    unsigned long long off[MAX_WORLD]; /* off[r] = records of the old ranks before r */
+    unsigned long long slice;          /* records per new rank (ceil(total / W_new); >= 1) */
+    int old_world, _pad;
+};
+__host__ __device__ __forceinline__ uint64_t remap_gid(const GidRemap& m, uint64_t gid) {
+    if (gid == ROOT_GID) return ROOT_GID;
+    const int r = (int)(gid >> 40);
+    const unsigned long long F = m.off[r < m.old_world ? r : 0] + (gid & ((1ull << 40) - 1ull));
+    return make_gid((int)(F / m.slice), F % m.slice);
+}
+__host__ __device__ __forceinline__ uint64_t remap_trec(const GidRemap& m, uint64_t t) {
+    return make_trec(remap_gid(m, (t >> 12) & GID_MASK), (uint32_t)(t & 0xFFFu));
+}
+
+/* one chunk of an old rank's frontier, with the trace records of those states (NULL without a trace) */
+struct ReshardParams {
+    const uint32_t* in;                /* n states of L::NW words */
+    const uint64_t* in_trace;          /* their records in the old numbering */
+    unsigned long long n;
+    uint32_t* out;                     /* frontier buffer 0: [0, out_split) in HBM, the rest at out_hi (spill) */
+    uint32_t* out_hi;
+    unsigned long long out_split, out_cap;
+    uint64_t* trace;                   /* record of kept state j goes to trace[trace_base + j] (NULL: no trace) */
+    unsigned long long trace_base, trace_cap;
+    const uint64_t* table;             /* this rank's seen-set, already filled from every old file */
+    unsigned long long table_cap;
+    const uint64_t* fp_tab;
+    RunCfg run;
+    int rank, owner_shift, level, _pad;
+    GidRemap remap;
+    unsigned long long* kept;          /* states this rank owns, over all chunks (their positions in buffer 0) */
+    unsigned long long* missing;       /* owned states not in the seen-set with the checkpoint's level */
+};
+/* Keep the states this rank owns — the expand kernel's fingerprint and owner rule — and append them to frontier buffer 0
+   (one atomic per warp), each with its trace record renumbered.  Every kept state must already be in the seen-set at the
+   checkpoint's level: a miss means the files disagree, and the host refuses the recovery. */
+template <class L> __global__ void reshard_frontier_kernel(const ReshardParams P) {
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long rounds = (P.n + stride - 1) / stride;
+    const int lane = threadIdx.x & 31;
+    unsigned long long miss = 0;
+    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (unsigned long long rd = 0; rd < rounds; rd++, i += stride) { /* whole warps stay in the loop: the ballot is warp-wide */
+        uint32_t w[L::NW];
+        bool mine = false;
+        if (i < P.n) {
+            for (int j = 0; j < L::NW; j++) w[j] = P.in[i * L::NW + j];
+            uint64_t fp = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
+            if (fp == 0) fp = 1;
+            mine = owner_of(fp, P.owner_shift) == P.rank;
+            if (mine && (int)(table_lookup(P.table, P.table_cap, fp, check_hash<L>(w, P.run.use_view != 0)) >> 56) != P.level) miss++;
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, mine);
+        if (!m) continue;
+        unsigned long long base = 0;
+        const int leader = __ffs(m) - 1;
+        if (lane == leader) base = atomicAdd(P.kept, (unsigned long long)__popc(m));
+        base = __shfl_sync(0xffffffffu, base, leader);
+        if (!mine) continue;
+        const unsigned long long pos = base + __popc(m & ((1u << lane) - 1u));
+        if (pos >= P.out_cap) continue; /* counted: the host reports the owned frontier's size */
+        uint32_t* dst = pos < P.out_split ? P.out + pos * L::NW : P.out_hi + (pos - P.out_split) * L::NW;
+        for (int j = 0; j < L::NW; j++) dst[j] = w[j];
+        if (P.trace && P.trace_base + pos < P.trace_cap) P.trace[P.trace_base + pos] = remap_trec(P.remap, P.in_trace[i]);
+    }
+    for (int o = 16; o; o >>= 1) miss += __shfl_xor_sync(0xffffffffu, miss, o);
+    if (lane == 0 && miss) atomicAdd(P.missing, miss);
+}
+
 /* ------------------------------------------------------------------ simulation mode (TLC `-simulate`)
    One thread per random walk from Init, `depth` states long at most; the invariant is checked on every state reached.
    The first violating (walk, depth) is kept (smallest walk index wins) and re-walked on the host for the trace. */

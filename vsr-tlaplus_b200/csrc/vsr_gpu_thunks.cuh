@@ -27,6 +27,8 @@ struct GpuOps {
     /* liveness pass (vsr_live.cuh): store a level's not-P states; one elimination sweep over store indices [first, first + n) */
     cudaError_t (*launch_live_collect)(const LiveParams&, int sms, cudaStream_t);
     cudaError_t (*launch_live_sweep)(const LiveParams&, int sms, cudaStream_t);
+    /* recovery on another number of ranks (vsr_ckpt.cu): keep this rank's share of one chunk of an old rank's frontier */
+    cudaError_t (*launch_reshard_frontier)(const ReshardParams&, int sms, cudaStream_t);
 };
 
 /* what a layout plug-in must have been compiled against: the version constant AND the shapes of the structs the kernels and the
@@ -82,13 +84,19 @@ template <class L> struct GpuThunks {
         live_sweep_kernel<L><<<(unsigned)(want < most ? want : most), 128, 0, st>>>(q);
         return cudaGetLastError();
     }
+    static cudaError_t launch_reshard_frontier(const ReshardParams& q, int sms, cudaStream_t st) {
+        if (!q.n) return cudaSuccess;
+        const unsigned long long want = (q.n + 255) / 256, most = (unsigned long long)sms * 8;
+        reshard_frontier_kernel<L><<<(unsigned)(want < most ? want : most), 256, 0, st>>>(q);
+        return cudaGetLastError();
+    }
     static uint32_t chk(const uint32_t* w, int use_view) { return check_hash<L>(w, use_view != 0); }
     static const GpuOps* get() {
         typedef ExpandCfg<L> Cfg;
         static const GpuOps ops = {chk, L::R, L::V, L::K, L::NW, L::BYTES, (int)(L::BYTES + sizeof(RecHdr)), sizeof(typename Cfg::Smem), Cfg::WARPS * 32,
                                    launch_expand, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate,
                                    Cfg::WARPS, Cfg::BLOCKS, Cfg::PASSES, Expander<L, false>::SROWS, launch_audit,
-                                   launch_live_collect, launch_live_sweep};
+                                   launch_live_collect, launch_live_sweep, launch_reshard_frontier};
         return &ops;
     }
 };

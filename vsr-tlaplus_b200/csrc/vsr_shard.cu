@@ -53,6 +53,12 @@ struct LevelMsg {
 };
 static_assert(sizeof(LevelMsg) <= VSR_GROUP_MSG_BYTES, "all-gather slot");
 
+struct RecoverMsg {
+    int32_t rc;
+    char msg[VSR_GROUP_MSG_BYTES - 4];
+};
+static_assert(sizeof(RecoverMsg) <= VSR_GROUP_MSG_BYTES, "all-gather slot");
+
 struct WalkMsg {
     uint64_t parent;
     uint32_t cand, ok;
@@ -272,7 +278,27 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     bool resumed = false;
     int rc;
     if (opts->recover_path) {
-        rc = vsr_engine_recover(e, rank_file(opts->recover_path).c_str(), &tot);
+        /* a checkpoint of this world: each rank reads its own file.  Of another world: each rank reads every old file and
+           keeps its share (vsr_ckpt.cu).  Every rank takes the same choice from the same files */
+        std::vector<std::string> old;
+        rc = ckpt_old_files(e, opts->recover_path, old);
+        if (!rc && old.empty()) rc = vsr_engine_recover(e, rank_file(opts->recover_path).c_str(), &tot);
+        else if (!rc) {
+            rc = ckpt_recover_resharded(e, old, &tot);
+            if (W > 1) { /* a share that does not fit fails on its rank only: all report the first failure, with its message */
+                RecoverMsg rm, rms[MAX_WORLD];
+                memset(&rm, 0, sizeof rm);
+                rm.rc = rc;
+                if (rc) memcpy(rm.msg, e->last_error, sizeof rm.msg - 1);
+                if (vsr_group_allgather(g, &rm, sizeof rm, rms)) return set_error(e, "%s", g->last_error);
+                for (int r = 0; r < W; r++)
+                    if (rms[r].rc) {
+                        if (!rc) snprintf(e->last_error, sizeof e->last_error, "%s", rms[r].msg);
+                        rc = rms[r].rc;
+                        break;
+                    }
+            }
+        }
         if (!rc) {
             resumed = true;
             level = e->level - 1; /* the loop's first pass stands at the checkpoint's level boundary without finishing a level */

@@ -175,7 +175,8 @@ class GpuEngine:
             want_trace: bool = True, part_states: int = 0, verbose: bool = False, checkpoint_path: Optional[str] = None,
             recover_path: Optional[str] = None, checkpoint_seconds: float = 0.0) -> ShardedResult:
         """checkpoint_path / recover_path: written / read at level boundaries (TLC -checkpoint / -recover); with several ranks
-        every rank uses ``<path>.rank<r>``"""
+        every rank uses ``<path>.rank<r>``.  recover_path may have been written by any number of ranks: every rank then reads
+        all the old files and keeps its own share.  Not with exchange="staged": that engine cannot run this loop."""
         o = self._opts
         o.max_depth, o.max_seconds, o.max_states = max_depth, max_seconds, max_states
         o.stop_on_violation, o.verbose = int(stop_on_violation), int(verbose)
@@ -296,7 +297,8 @@ def check_sharded(mc: "ck.ModelChecker", group: Group, device: int = 0, table_ca
                   inbox_records: int = 0, part_states: int = 0, keep_trace: bool = True, check_deadlock: bool = False,
                   coverage: bool = False, **run_kw) -> ShardedResult:
     """One call per rank: engine + inbox + BFS + teardown; on a violation rank 0's result carries the literal trace.
-    coverage: count TLC's action coverage (ShardedResult.coverage, the job's totals on every rank)."""
+    coverage: count TLC's action coverage (ShardedResult.coverage, the job's totals on every rank).  recover_path= (in
+    run_kw) continues a checkpoint written by any number of ranks."""
     eng = GpuEngine(mc, group.rank, group.world, device=device, table_capacity=table_capacity, frontier_capacity=frontier_capacity,
                     inbox_records=inbox_records, keep_trace=keep_trace, check_deadlock=check_deadlock, group=group, coverage=coverage)
     res = None
