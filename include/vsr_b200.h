@@ -355,18 +355,26 @@ int vsr_replay_candidates(const VsrModel* m, const uint32_t* cands, int n, void*
                           size_t trace_cap);
 
 /* ---- simulation mode: TLC `-simulate [-depth N]` (the reference's README.md:22 recommends it for the defect).
- * num_walks random behaviours from Init of at most `depth` states (TLC's default 100), uniformly random among the
- * enabled (action, binding) pairs at every step, invariant checked on every state; one GPU thread per walk.  Returns 12
- * and the violating behaviour (literal value names, re-walked on the host) if one walk hits a violation. */
+ * num_walks random behaviours from Init of at most `depth` states (TLC's default 100), one GPU thread per walk.  Each step
+ * is drawn uniformly among the enabled candidates of the current state: one per (action, binding) pair, except that under
+ * SYMMETRY one ReceiveClientRequest candidate stands for every value not yet requested.  The invariant is checked on
+ * every state after Init.  The reported walk is the smallest walk index that violates the invariant (returns 12) or, with
+ * check_deadlock, reaches a state without successors before the depth bound (returns 11, TLC's "Deadlock reached"); it is
+ * re-walked on the host and returned as a literal behaviour (literal value names).  Walks ending in a state without
+ * successors are counted in dead_ends either way. */
 typedef struct VsrSimOpts {
     int32_t device, depth;
     uint64_t num_walks, seed;
-    uint64_t probe_walks;   /* optional cross-check: for walks 0 .. probe_walks-1 the device reports ... */
+    uint64_t probe_walks;   /* optional cross-check: for walks 0 .. min(probe_walks, num_walks)-1 the device reports ... */
     uint64_t* probe_out;    /* ... [2w] = bytewise FP64 of the walk's last state (all words), [2w+1] = transitions taken; NULL = off */
+    int32_t check_deadlock; /* TLC checks deadlock unless -deadlock is given; 0 = only count walks without successors */
+    int32_t _pad;
 } VsrSimOpts;
 typedef struct VsrSimStats {
-    uint64_t walks, steps, dead_ends, violating_walk;
-    int32_t rc, violation_depth, trace_len, _pad;
+    uint64_t walks, steps, dead_ends;
+    uint64_t violating_walk;          /* the reported walk: its index ... */
+    int32_t rc, violation_depth;      /* ... and the depth (Init = 1) of its violating / successor-less last state */
+    int32_t trace_len, _pad;
     double kernel_ms, seconds_total;
 } VsrSimStats;
 int vsr_simulate(const VsrModel* m, const VsrSimOpts* opts, VsrSimStats* out, void* trace_out, uint8_t* trace_actions,

@@ -25,14 +25,15 @@ def test_library_exports_every_declared_symbol(pkg):
 
 def test_struct_mirrors_match_c_sizes(pkg, tmp_path):
     src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include "vsr_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(VsrFlatState), sizeof(VsrMsg),'
-                   ' sizeof(VsrModelInfo), sizeof(VsrRunOpts), sizeof(VsrStats), sizeof(VsrLevelInfo)); return 0;}\n')
+    src.write_text('#include <stdio.h>\n#include "vsr_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(VsrFlatState), sizeof(VsrMsg),'
+                   ' sizeof(VsrModelInfo), sizeof(VsrRunOpts), sizeof(VsrStats), sizeof(VsrLevelInfo), sizeof(VsrSimOpts),'
+                   ' sizeof(VsrSimStats)); return 0;}\n')
     exe = tmp_path / "sz"
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
     sizes = [int(x) for x in subprocess.check_output([str(exe)]).split()]
     ck = pkg.checker
     assert sizes == [C.sizeof(ck.VsrFlatState), C.sizeof(ck.VsrMsg), C.sizeof(ck.VsrModelInfo), C.sizeof(ck.VsrRunOpts),
-                     C.sizeof(ck.VsrStats), C.sizeof(ck.VsrLevelInfo)]
+                     C.sizeof(ck.VsrStats), C.sizeof(ck.VsrLevelInfo), C.sizeof(ck.VsrSimOpts), C.sizeof(ck.VsrSimStats)]
 
 
 def test_shipped_cfg_loads(pkg):

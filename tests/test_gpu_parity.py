@@ -234,63 +234,6 @@ def test_view_ties_resolve_to_smallest_aux_key(pkg):
         eng.close()
 
 
-def test_simulation_mode_walks_like_the_host_and_replays_violations(pkg):
-    """TLC's `-simulate` (the reference's README recommends it): one GPU thread per random walk.
-    (1) device walks == host walks: for the first 2000 walks the device reports (fingerprint of the last state, transitions
-        taken); the host re-walks them with the same generator through the C ABI and must agree exactly;
-    (2) uniform random walks essentially never hit the real invariants' violations (28e6 host walks of R=3,V=2,L=1 found
-        none), so the violation path is exercised with the library's test-hook invariant (mask 256: "no replica has
-        committed every value"): the violating walk is re-walked on the host and must be a literal behaviour of the spec
-        per the ORACLE, violating only in its last state;
-    (3) same seed, same answer; no violation reported where none exists."""
-    lib = pkg.load_library()
-    h = C.c_void_p()
-    err = C.create_string_buffer(256)
-    assert lib.vsr_model_create(3, 1, 2, 2, 0, 1, 1, 1, C.byref(h), err, len(err)) == 0
-    mc = pkg.ModelChecker(h, lib)
-    st, trace = mc.simulate(num_walks=1 << 16, depth=40, seed=11, probe_walks=2000)
-    assert st.rc == 0 and trace == [] and st.steps > 0 and st.dead_ends >= 0
-    nv = pkg.ModelChecker.from_constants(3, 2, 2, view=False)  # same layout, fingerprint over all words
-    for w, (fp, nsteps) in enumerate(mc.last_probe):
-        cands, viol = mc.walk(11, w, 40)
-        assert viol == 0 and nsteps == len(cands), w
-        cur = mc.init_state()
-        for c in cands:
-            en = (C.c_uint32 * 1024)()
-            n = lib.vsr_enabled_candidates(mc._h, (C.c_uint8 * mc.state_bytes).from_buffer_copy(cur), en, 1024)
-            succ = mc.successors(cur)
-            cur = succ[[int(en[i]) for i in range(n)].index(c)][0]
-        buf = (C.c_uint8 * mc.state_bytes).from_buffer_copy(cur)
-        assert nv._lib.vsr_fingerprint_bytewise(nv._h, buf) == fp, w
-        if w >= 300:
-            break
-    # (2) the violation path, through the test-hook invariant
-    h2 = C.c_void_p()
-    assert lib.vsr_model_create(3, 1, 1, 1, 0, 0, 1, 256, C.byref(h2), err, len(err)) == 0
-    hook = pkg.ModelChecker(h2, lib)
-    st, trace = hook.simulate(num_walks=1 << 16, depth=40, seed=5)
-    assert st.rc == 12 and len(trace) == st.violation_depth and trace[0][0] == "Initial predicate"
-    cands, viol = hook.walk(5, int(st.violating_walk), 40)
-    assert viol == st.violation_depth and len(cands) == viol - 1
-    q = orc.params(3, 1, 1, symmetry=False)
-    L = orc.lib()
-    flats = [hook.unpack(s) for _, s in trace]
-    for i in range(len(flats) - 1):
-        cap = 256
-        succ = (pkg.checker.VsrFlatState * cap)()
-        acts = (C.c_int * cap)()
-        n = L.orc_successors_flat(q, C.byref(flats[i]), succ, acts, cap)
-        want = orc.digests_full_of(q, (pkg.checker.VsrFlatState * 1)(flats[i + 1]))[0]
-        got = orc.digests_full_of(q, succ)[:n]
-        assert any(g == want and pkg.ACTION_NAMES[acts[k]] == trace[i + 1][0] for k, g in enumerate(got)), f"step {i + 1}"
-    assert max(f.rep[r].commit for f in flats[-1:] for r in range(3)) == 1
-    assert all(max(f.rep[r].commit for r in range(3)) == 0 for f in flats[:-1])
-    # (3) determinism
-    st2, trace2 = hook.simulate(num_walks=1 << 16, depth=40, seed=5)
-    assert (st2.violating_walk, st2.violation_depth, st2.steps) == (st.violating_walk, st.violation_depth, st.steps)
-    assert [s for _, s in trace2] == [s for _, s in trace]
-
-
 def test_frontier_spill_and_odd_capacities_give_the_same_exploration(pkg):
     """BASELINE configs[3]'s capacity path at test size: 700 frontier states in HBM, the rest of every level in pinned host
     memory (levels of up to thousands of states: most of them straddle the boundary), and a seen-set whose capacity is not a

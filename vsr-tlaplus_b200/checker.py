@@ -143,7 +143,7 @@ class VsrLiveStats(C.Structure):
 
 class VsrSimOpts(C.Structure):
     _fields_ = [("device", C.c_int32), ("depth", C.c_int32), ("num_walks", C.c_uint64), ("seed", C.c_uint64),
-                ("probe_walks", C.c_uint64), ("probe_out", C.POINTER(C.c_uint64))]
+                ("probe_walks", C.c_uint64), ("probe_out", C.POINTER(C.c_uint64)), ("check_deadlock", C.c_int32), ("_pad", C.c_int32)]
 
 
 class VsrSimStats(C.Structure):
@@ -629,10 +629,16 @@ class ModelChecker:
         res.coverage = self._coverage_of(o)
         return res
 
-    def simulate(self, num_walks: int = 1 << 20, depth: int = 100, seed: int = 1, device: int = 0, probe_walks: int = 0):
+    def simulate(self, num_walks: int = 1 << 20, depth: int = 100, seed: int = 1, device: int = 0, probe_walks: int = 0,
+                 deadlock: Optional[bool] = None):
         """TLC's `-simulate -depth N`: random behaviours on the GPU.  Returns (VsrSimStats, trace) — the trace is the
-        violating behaviour [(action name, packed state)] when rc == 12, else []."""
-        o = VsrSimOpts(device=device, depth=depth, num_walks=num_walks, seed=seed)
+        reported behaviour [(action name, packed state)] when rc == 12 (invariant violated) or 11 (deadlock), else [].
+        deadlock: report a walk that reaches a state without successors before the depth bound; None = CHECK_DEADLOCK of
+        the cfg when it has one, otherwise off (as run_opts).  last_probe: (fingerprint of the last state, transitions)
+        of walks 0 .. min(probe_walks, num_walks) - 1."""
+        if deadlock is None:
+            deadlock = int(self.info.check_deadlock) == 1
+        o = VsrSimOpts(device=device, depth=depth, num_walks=num_walks, seed=seed, check_deadlock=int(deadlock))
         probe = (C.c_uint64 * max(2 * probe_walks, 1))()
         if probe_walks:
             o.probe_walks, o.probe_out = probe_walks, probe
@@ -645,7 +651,7 @@ class ModelChecker:
         if rc == 153:
             raise VsrError(rc, "no usable CUDA device: simulation runs on the GPU only")
         raw, sb = bytes(tr), self.state_bytes
-        self.last_probe = [(int(probe[2 * i]), int(probe[2 * i + 1])) for i in range(probe_walks)]  # (fp of last state, transitions)
+        self.last_probe = [(int(probe[2 * i]), int(probe[2 * i + 1])) for i in range(min(probe_walks, num_walks))]  # (fp of last state, transitions)
         return st, [(ACTION_NAMES[acts[i]], raw[i * sb:(i + 1) * sb]) for i in range(int(st.trace_len))]
 
     def walk(self, seed: int, walk: int, depth: int):

@@ -610,8 +610,9 @@ uint64_t vsr_engine_collected(const VsrEngine* e, int level, void* host_out, uin
     return n;
 }
 
-/* TLC `-simulate`: random walks on the GPU; a violating walk is re-walked on the host (same generator, same step
-   function) and returned as a literal behaviour. */
+/* TLC `-simulate`: random walks on the GPU.  The reported walk — the smallest walk index that violates the invariant or,
+   with check_deadlock, reaches a state without successors before the depth bound — is re-walked on the host (same
+   generator, same step function), checked to end as the device says, and returned as a literal behaviour. */
 int vsr_simulate(const VsrModel* m, const VsrSimOpts* o, VsrSimStats* out, void* trace_out, uint8_t* trace_actions, size_t trace_cap) {
     if (!m || !o || !out) return VSR_RC_ERROR;
     memset(out, 0, sizeof *out);
@@ -622,17 +623,19 @@ int vsr_simulate(const VsrModel* m, const VsrSimOpts* o, VsrSimStats* out, void*
     if (cudaSetDevice(o->device) != cudaSuccess) return VSR_RC_SYSTEM;
     const double t0 = now_s();
     unsigned long long* d = nullptr;
-    if (cudaMalloc(&d, 24) != cudaSuccess) return VSR_RC_SYSTEM;
-    unsigned long long init[3] = {~0ull, 0, 0};
-    cudaMemcpy(d, init, 24, cudaMemcpyHostToDevice);
+    if (cudaMalloc(&d, 32) != cudaSuccess) return VSR_RC_SYSTEM;
+    unsigned long long init[4] = {~0ull, 0, 0, ~0ull};
+    cudaMemcpy(d, init, 32, cudaMemcpyHostToDevice);
     SimParams q;
     q.num_walks = o->num_walks;
     q.seed = o->seed;
     q.depth = o->depth > 0 ? o->depth : 100; /* TLC's default simulation depth */
+    q.check_deadlock = o->check_deadlock != 0;
     q.run = m->run;
     q.first_bad = d;
     q.steps = d + 1;
     q.dead_ends = d + 2;
+    q.first_dead = d + 3;
     unsigned long long* dprobe = nullptr;
     uint64_t* dtab = nullptr;
     q.probe_walks = (o->probe_out && o->probe_walks) ? o->probe_walks : 0;
@@ -654,8 +657,8 @@ int vsr_simulate(const VsrModel* m, const VsrSimOpts* o, VsrSimStats* out, void*
     if (ce != cudaSuccess || cudaEventSynchronize(b) != cudaSuccess) { cudaFree(d); return VSR_RC_SYSTEM; }
     float ms = 0;
     cudaEventElapsedTime(&ms, a, b);
-    unsigned long long h[3];
-    cudaMemcpy(h, d, 24, cudaMemcpyDeviceToHost);
+    unsigned long long h[4];
+    cudaMemcpy(h, d, 32, cudaMemcpyDeviceToHost);
     if (q.probe_walks) cudaMemcpy(o->probe_out, dprobe, q.probe_walks * 16, cudaMemcpyDeviceToHost);
     cudaFree(dprobe);
     cudaFree(dtab);
@@ -667,10 +670,13 @@ int vsr_simulate(const VsrModel* m, const VsrSimOpts* o, VsrSimStats* out, void*
     out->dead_ends = h[2];
     out->kernel_ms = ms;
     int rc = 0;
-    if (h[0] != ~0ull) {
-        rc = VSR_RC_VIOLATION;
-        out->violating_walk = h[0] >> 16;
-        out->violation_depth = (int)(h[0] & 0xFFFF);
+    if (h[0] != ~0ull || h[3] != ~0ull) {
+        /* walks are numbered in the high bits, and no walk both violates and dead-ends: the smaller key is the smaller walk */
+        const bool dead = h[3] < h[0];
+        const unsigned long long key = dead ? h[3] : h[0];
+        rc = dead ? VSR_RC_DEADLOCK : VSR_RC_VIOLATION;
+        out->violating_walk = key >> 16;
+        out->violation_depth = (int)(key & 0xFFFF);
         /* re-walk on the host */
         const ModelOps* ops = m->ops;
         std::vector<uint32_t> cands;
@@ -683,8 +689,10 @@ int vsr_simulate(const VsrModel* m, const VsrSimOpts* o, VsrSimStats* out, void*
             memcpy(cur, nxt, ops->bytes);
             cands.push_back((uint32_t)c);
         }
-        if (rc == VSR_RC_VIOLATION && !ops->invariant(&m->run, cur)) rc = VSR_RC_ERROR; /* host and device disagree */
-        if (rc == VSR_RC_VIOLATION && trace_out) {
+        /* host and device disagree unless the last state violates / has no enabled candidate */
+        if (rc == VSR_RC_VIOLATION && !ops->invariant(&m->run, cur)) rc = VSR_RC_ERROR;
+        if (rc == VSR_RC_DEADLOCK && ops->random_enabled(&m->run, cur, &rng) >= 0) rc = VSR_RC_ERROR;
+        if (rc != VSR_RC_ERROR && trace_out) {
             const int n = vsr_replay_candidates(m, cands.data(), (int)cands.size(), trace_out, trace_actions, trace_cap);
             out->trace_len = n > 0 ? n : 0;
         }

@@ -1174,12 +1174,14 @@ template <class L> __global__ void reshard_frontier_kernel(const ReshardParams P
 
 /* ------------------------------------------------------------------ simulation mode (TLC `-simulate`)
    One thread per random walk from Init, `depth` states long at most; the invariant is checked on every state reached.
-   The first violating (walk, depth) is kept (smallest walk index wins) and re-walked on the host for the trace. */
+   The first violating (walk, depth) is kept (smallest walk index wins), and with check_deadlock the first (walk, depth) of
+   a state without successors before the bound; the host re-walks the smaller of the two for the trace. */
 struct SimParams {
     unsigned long long num_walks, seed;
-    int depth;
+    int depth, check_deadlock;
     RunCfg run;
     unsigned long long* first_bad; /* walk << 16 | depth of the state that violates (~0 = none) */
+    unsigned long long* first_dead; /* walk << 16 | depth of the state without successors (~0 = none); check_deadlock only */
     unsigned long long* steps;     /* transitions taken */
     unsigned long long* dead_ends; /* walks that stopped in a state without successors */
     unsigned long long* probe_out; /* optional: for walks 0 .. probe_walks-1, fingerprint of the last state and transitions taken */
@@ -1195,7 +1197,11 @@ template <class L> __global__ void simulate_kernel(const SimParams Q) {
         unsigned long long mysteps = 0;
         for (int d = 2; d <= Q.depth; d++) {
             const int cand = Ops<L>::random_enabled(Q.run, (const uint32_t*)a, rng);
-            if (cand < 0) { dead++; break; }
+            if (cand < 0) {
+                dead++;
+                if (Q.check_deadlock) atomicMin(Q.first_dead, (wk << 16) | (unsigned long long)(d - 1));
+                break;
+            }
             if (Ops<L>::template step<true>(Q.run, (const uint32_t*)a, cand, (uint32_t*)b) <= 0) break;
             for (int j = 0; j < L::NW; j++) a[j] = b[j];
             steps++;
