@@ -100,22 +100,6 @@ int io_error(VsrEngine* e, const char* what, const char* path) {
     return VSR_RC_SYSTEM;
 }
 
-/* frontier states [first, first + n) of buffer `buf` <-> host: the part in HBM by cudaMemcpy, the spilled part directly */
-int frontier_to_host(VsrEngine* e, int buf, uint64_t first, uint64_t n, uint8_t* host) {
-    const uint64_t S = (uint64_t)e->g->bytes;
-    const uint64_t in_dev = first < e->frontier_cap ? std::min(n, e->frontier_cap - first) : 0;
-    if (in_dev) CK(cudaMemcpy(host, (const uint8_t*)e->frontier[buf] + first * S, in_dev * S, cudaMemcpyDeviceToHost));
-    if (n > in_dev) memcpy(host + in_dev * S, (const uint8_t*)e->frontier_host[buf] + (first + in_dev - e->frontier_cap) * S, (n - in_dev) * S);
-    return 0;
-}
-int frontier_from_host(VsrEngine* e, int buf, uint64_t first, uint64_t n, const uint8_t* host) {
-    const uint64_t S = (uint64_t)e->g->bytes;
-    const uint64_t in_dev = first < e->frontier_cap ? std::min(n, e->frontier_cap - first) : 0;
-    if (in_dev) CK(cudaMemcpy((uint8_t*)e->frontier[buf] + first * S, host, in_dev * S, cudaMemcpyHostToDevice));
-    if (n > in_dev) memcpy((uint8_t*)e->frontier_host[buf] + (first + in_dev - e->frontier_cap) * S, host + in_dev * S, (n - in_dev) * S);
-    return 0;
-}
-
 constexpr uint64_t IO_CHUNK = 64ull << 20; /* bytes per host staging round */
 
 bool header_ok(const CkptHeader& h) {
@@ -183,15 +167,14 @@ int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals
         host.resize(per * S);
         for (uint64_t first = 0; first < e->n_cur; first += per) {
             const uint64_t n = std::min(per, e->n_cur - first);
-            int rc = frontier_to_host(e, e->cur, first, n, host.data());
-            if (rc) return rc;
+            CK(e->frontier[e->cur].to_host(first, n, host.data()));
             if (fwrite(host.data(), S, n, out.f) != n) return io_error(e, "cannot write", tmp.c_str());
         }
     }
     /* 2. the seen-set's entries, compacted into the idle frontier buffer (its HBM part) chunk by chunk */
     {
-        uint64_t* scratch = (uint64_t*)e->frontier[e->cur ^ 1];
-        const uint64_t slots_per_pass = std::max<uint64_t>(64, e->frontier_cap * S / 16);
+        uint64_t* scratch = (uint64_t*)e->frontier[e->cur ^ 1].hbm;
+        const uint64_t slots_per_pass = std::max<uint64_t>(64, e->frontier[e->cur ^ 1].hbm_rows * S / 16);
         unsigned long long* dcount = &e->ctr->work_next; /* scratch word: the level's counters are reset when it opens */
         uint64_t written = 0;
         for (uint64_t first = 0; first < e->table_cap; first += slots_per_pass) {
@@ -262,7 +245,7 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
         snprintf(e->last_error, sizeof e->last_error, "recover: %s is rank %d of %d, this engine is rank %d of %d", path, h.rank, h.world, e->rank, e->world);
         return VSR_RC_CONFIG_ERROR;
     }
-    if (h.n_cur > e->frontier_cap + e->frontier_host_cap || h.n_entries > e->table_cap - e->table_cap / 8 || (h.n_trace && e->trace && h.n_trace > e->trace_cap)) {
+    if (h.n_cur > e->frontier[0].capacity() || h.n_entries > e->table_cap - e->table_cap / 8 || (h.n_trace && e->trace && h.n_trace > e->trace_cap)) {
         snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (recover): the checkpoint holds %llu frontier states and %llu seen-set entries",
                  (unsigned long long)h.n_cur, (unsigned long long)h.n_entries);
         return VSR_RC_TOO_LARGE;
@@ -284,14 +267,13 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
         for (uint64_t first = 0; first < h.n_cur; first += per) {
             const uint64_t n = std::min(per, h.n_cur - first);
             if (fread(host.data(), S, n, in.f) != n) return io_error(e, "truncated", path);
-            rc = frontier_from_host(e, 0, first, n, host.data());
-            if (rc) return rc;
+            CK(e->frontier[0].from_host(first, n, host.data()));
         }
     }
     /* 2. the seen-set, re-inserted through the idle frontier buffer */
     {
-        uint64_t* scratch = (uint64_t*)e->frontier[1];
-        const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>(IO_CHUNK / 16, e->frontier_cap * S / 16));
+        uint64_t* scratch = (uint64_t*)e->frontier[1].hbm;
+        const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>(IO_CHUNK / 16, e->frontier[1].hbm_rows * S / 16));
         unsigned long long* dbad = &e->ctr->work_next;
         CK(cudaMemsetAsync(dbad, 0, 8, e->stream));
         host.resize(per * 16);
@@ -442,8 +424,8 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
     std::vector<uint8_t> host;
     unsigned long long* d0 = &e->ctr->work_next; /* scratch words: the level's counters are reset when it opens */
     unsigned long long* d1 = &e->ctr->drain_next;
-    uint8_t* scratch = (uint8_t*)e->frontier[1];
-    const uint64_t scratch_bytes = e->frontier_cap * S;
+    uint8_t* scratch = (uint8_t*)e->frontier[1].hbm;
+    const uint64_t scratch_bytes = e->frontier[1].hbm_rows * S;
     /* 3. the seen-set entries this rank owns.  Chunks of at most 1/16 of the table: the load is checked after every chunk,
        so a share that does not fit stops at 15/16 load, where inserts still end */
     const uint64_t limit = e->table_cap - e->table_cap / 8;
@@ -488,7 +470,7 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
     /* 4. the frontier states this rank owns, into buffer 0, with their trace records after this rank's slice */
     uint64_t kept = 0;
     {
-        const uint64_t fcap_total = e->frontier_cap + e->frontier_host_cap;
+        const uint64_t fcap_total = e->frontier[0].capacity();
         const bool tr = e->trace && h[0].keep_trace;
         const uint64_t per = std::max<uint64_t>(1, (std::min(IO_CHUNK, scratch_bytes) - 16) / (S + 8));
         const uint64_t tr_off = (per * S + 15) & ~15ull;
@@ -496,9 +478,7 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
         memset(&q, 0, sizeof q);
         q.in = (const uint32_t*)scratch;
         q.in_trace = tr ? (const uint64_t*)(scratch + tr_off) : nullptr;
-        q.out = e->frontier[0];
-        q.out_hi = e->frontier_host[0];
-        q.out_split = e->frontier_host_cap ? e->frontier_cap : ~0ull;
+        q.out = e->frontier[0].view();
         q.out_cap = fcap_total;
         q.trace = tr ? e->trace : nullptr;
         q.trace_base = cur_base;

@@ -41,10 +41,7 @@ struct VsrEngine {
     /* device memory */
     uint64_t* table = nullptr;
     uint64_t table_cap = 0;
-    uint32_t* frontier[2] = {nullptr, nullptr};
-    uint64_t frontier_cap = 0;        /* states per buffer in HBM */
-    uint32_t* frontier_host[2] = {nullptr, nullptr}; /* continuation of each buffer in pinned host memory (spill) */
-    uint64_t frontier_host_cap = 0;
+    vsr::SpillBuffer frontier[2];     /* states; each continues in pinned host memory with frontier_host_capacity */
     uint64_t* trace = nullptr;
     uint64_t trace_cap = 0;
     vsr::DevCounters* ctr = nullptr;
@@ -78,9 +75,7 @@ struct VsrEngine {
        kernels are launched without the counters: ExpandParams::cover stays NULL) */
     VsrCoverage* cov = nullptr;
     /* liveness store (models with a property; vsr_live.cu): the not-P states of every finished level, grouped by level */
-    uint32_t* live_words = nullptr;      /* [0, live_dev_cap) in HBM */
-    uint32_t* live_words_host = nullptr; /* the rest in pinned host memory mapped into the device */
-    uint64_t live_cap = 0, live_dev_cap = 0;
+    vsr::SpillBuffer live_words;         /* the stored states; capacity() = the store's */
     unsigned long long* live_ids = nullptr; /* BFS local id per stored state */
     uint64_t* live_index = nullptr;      /* {fp, (store index + 1) << 32 | check} */
     uint64_t live_index_cap = 0;

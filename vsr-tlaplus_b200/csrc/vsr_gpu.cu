@@ -45,15 +45,11 @@ int engine_reset_level(VsrEngine* e) {
 
 void fill_params(VsrEngine* e, ExpandParams& p) {
     memset(&p, 0, sizeof p);
-    p.in = e->frontier[e->cur];
+    p.in = e->frontier[e->cur].view();
     p.n_in = e->n_cur;
     p.in_base = e->cur_base;
-    p.in_hi = e->frontier_host[e->cur];
-    p.in_split = e->frontier_host_cap ? e->frontier_cap : ~0ull;
-    p.out = e->frontier[e->cur ^ 1];
-    p.out_hi = e->frontier_host[e->cur ^ 1];
-    p.out_split = e->frontier_host_cap ? e->frontier_cap : ~0ull;
-    p.out_cap = e->frontier_cap + e->frontier_host_cap;
+    p.out = e->frontier[e->cur ^ 1].view();
+    p.out_cap = e->frontier[e->cur ^ 1].capacity();
     p.out_base = e->next_base;
     p.table = e->table;
     p.table_cap = e->table_cap;
@@ -187,19 +183,14 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     if (!fcap) fcap = (uint64_t)(free_b * (live ? 0.15 : 0.40)) / (2 * S);
     if (fcap < 64) fcap = 64;
     e->table_cap = tcap;
-    e->frontier_cap = fcap;
     e->trace_cap = opts->keep_trace ? tcap - tcap / 8 + 64 : 0; /* one record per distinct state, up to the seen-set's load limit */
     e->tie_cap = 1 << 16;
     if ((ce = cudaMallocAsync((void**)&e->table, tcap * 16, e->stream)) != cudaSuccess) return bail("cudaMalloc(seen-set)", ce);
     if ((ce = cudaMemsetAsync(e->table, 0, tcap * 16, e->stream)) != cudaSuccess) return bail("memset", ce);
     for (int i = 0; i < 2; i++)
-        if ((ce = cudaMallocAsync((void**)&e->frontier[i], fcap * S, e->stream)) != cudaSuccess) return bail("cudaMalloc(frontier)", ce);
-    if (opts->frontier_host_capacity) { /* spill: each frontier buffer continues in pinned, device-mapped host memory */
-        e->frontier_host_cap = opts->frontier_host_capacity;
-        for (int i = 0; i < 2; i++)
-            if ((ce = cudaHostAlloc((void**)&e->frontier_host[i], e->frontier_host_cap * S, cudaHostAllocPortable | cudaHostAllocMapped)) != cudaSuccess)
-                return bail("cudaHostAlloc(frontier spill)", ce);
-    }
+        if ((ce = e->frontier[i].alloc_hbm(fcap, S, e->stream)) != cudaSuccess) return bail("cudaMalloc(frontier)", ce);
+    for (int i = 0; i < 2; i++) /* spill: each frontier buffer continues in pinned, device-mapped host memory */
+        if ((ce = e->frontier[i].alloc_host(opts->frontier_host_capacity)) != cudaSuccess) return bail("cudaHostAlloc(frontier spill)", ce);
     if (e->trace_cap && (ce = cudaMallocAsync((void**)&e->trace, e->trace_cap * 8, e->stream)) != cudaSuccess) return bail("cudaMalloc(trace)", ce);
     if ((ce = cudaMallocAsync((void**)&e->ctr, sizeof(LevelCounters), e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->ties, e->tie_cap * (size_t)e->g->tie_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
@@ -207,7 +198,7 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     if ((ce = cudaMallocAsync((void**)&e->init_rec, e->g->rec_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMemcpyAsync(e->fp_tab, fp64_table(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess) return bail("memcpy", ce);
     e->st.table_capacity = tcap;
-    e->st.frontier_capacity = fcap + e->frontier_host_cap;
+    e->st.frontier_capacity = e->frontier[0].capacity();
     e->st.bytes_table = tcap * 16;
     e->st.bytes_frontier = 2 * fcap * S;
     e->st.bytes_h2d += 8 * 256 * 8;
@@ -226,10 +217,7 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
 void vsr_engine_destroy(VsrEngine* e) {
     if (!e) return;
     if (e->stream) cudaFreeAsync(e->table, e->stream); else cudaFree(e->table);
-    if (e->stream) cudaFreeAsync(e->frontier[0], e->stream); else cudaFree(e->frontier[0]);
-    if (e->stream) cudaFreeAsync(e->frontier[1], e->stream); else cudaFree(e->frontier[1]);
-    for (int i = 0; i < 2; i++)
-        if (e->frontier_host[i]) cudaFreeHost(e->frontier_host[i]);
+    for (SpillBuffer& f : e->frontier) f.release(e->stream);
     if (e->stream) cudaFreeAsync(e->trace, e->stream); else cudaFree(e->trace);
     if (e->stream) cudaFreeAsync(e->ctr, e->stream); else cudaFree(e->ctr);
     if (e->stream) cudaFreeAsync(e->ties, e->stream); else cudaFree(e->ties);
@@ -283,14 +271,7 @@ int vsr_engine_step(VsrEngine* e, uint64_t first, uint64_t count, int parity, co
     else if (count > e->n_cur - first) count = e->n_cur - first;
     ExpandParams p;
     fill_params(e, p);
-    if (first < p.in_split || !e->frontier_host_cap) {
-        p.in += first * (uint64_t)e->g->nw;
-        if (e->frontier_host_cap) p.in_split -= first;
-    } else { /* this part lies entirely in the host part of the frontier */
-        p.in = p.in_hi + (first - p.in_split) * (uint64_t)e->g->nw;
-        p.in_hi = nullptr;
-        p.in_split = ~0ull;
-    }
+    p.in = p.in.from(first, e->g->nw);
     p.n_in = count;
     p.in_base += first;
     uint64_t drain_total = 0;
@@ -357,7 +338,7 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
     CK(cudaMemcpyAsync(&lc, e->ctr, ctr_bytes, cudaMemcpyDeviceToHost, e->stream));
     e->st.bytes_d2h += ctr_bytes;
     CK(cudaStreamSynchronize(e->stream));
-    const uint64_t fcap_total = e->frontier_cap + e->frontier_host_cap;
+    const uint64_t fcap_total = e->frontier[e->cur ^ 1].capacity();
     if (c.tie_count > 0 && c.tie_count <= e->tie_cap && !c.overflow && c.out_count <= fcap_total) {
         /* SURVEY H2: same-level states with equal VIEW but different aux variables.  Keep, per fingerprint, the
            smallest (aux_key, parent, candidate) among the late arrivals, sorted by fingerprint, and let the patch
@@ -493,10 +474,7 @@ uint64_t vsr_engine_frontier_size(const VsrEngine* e) { return e->n_cur; }
 
 int vsr_engine_read_frontier(VsrEngine* e, uint64_t first, uint64_t n, void* host_out) {
     if (first + n > e->n_cur) return VSR_RC_ERROR;
-    const uint64_t S = (uint64_t)e->g->bytes;
-    const uint64_t in_dev = first < e->frontier_cap ? std::min(n, e->frontier_cap - first) : 0; /* the rest is in the host part (spill) */
-    if (in_dev) CK(cudaMemcpy(host_out, (const uint8_t*)e->frontier[e->cur] + first * S, in_dev * S, cudaMemcpyDeviceToHost));
-    if (n > in_dev) memcpy((uint8_t*)host_out + in_dev * S, (const uint8_t*)e->frontier_host[e->cur] + (first + in_dev - e->frontier_cap) * S, (n - in_dev) * S);
+    CK(e->frontier[e->cur].to_host(first, n, host_out));
     return 0;
 }
 
@@ -537,11 +515,9 @@ int vsr_engine_audit_level(VsrEngine* e, VsrLevelAudit* out) {
     CK(cudaMallocAsync((void**)&d, sizeof(AuditSums), e->stream));
     ExpandParams p;
     fill_params(e, p);
-    p.out = e->frontier[e->cur]; /* the level just finished, read as the expand kernel wrote it (host part included) */
-    p.out_hi = e->frontier_host[e->cur];
     p.level = e->level;
     cudaError_t ce = cudaMemsetAsync(d, 0, sizeof(AuditSums), e->stream);
-    if (ce == cudaSuccess) ce = e->g->launch_audit(p, e->n_cur, d, e->sms, e->stream);
+    if (ce == cudaSuccess) ce = e->g->launch_audit(p, e->frontier[e->cur].view(), e->n_cur, d, e->sms, e->stream);
     AuditSums h;
     memset(&h, 0, sizeof h);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(&h, d, sizeof h, cudaMemcpyDeviceToHost, e->stream);

@@ -30,6 +30,7 @@
 
 #include "../../include/vsr_flat.h" /* VSR_ACT_*, VSR_NUM_ACTIONS */
 #include "vsr_actions.h"
+#include "vsr_spill.cuh"
 
 namespace vsr {
 
@@ -83,18 +84,12 @@ constexpr int MAX_WORLD = 8;
 
 
 struct ExpandParams {
-    const uint32_t* in;          /* current frontier, n_in states of L::NW words */
+    SpillRows in;                /* current frontier, n_in states of L::NW words (both frontiers may spill: vsr_spill.cuh) */
     unsigned long long n_in;
-    unsigned long long in_base;  /* local id of in[0] */
-    /* frontier spill (BASELINE configs[3]): a frontier buffer may continue in pinned host memory once its part in HBM is full.
-       States [0, in_split) of this launch's view are at `in`, the rest at in_hi (NULL / ~0: no spill); same for out. */
-    const uint32_t* in_hi;
-    unsigned long long in_split;
-    uint32_t* out;               /* next frontier */
-    uint32_t* out_hi;
-    unsigned long long out_split;
+    unsigned long long in_base;  /* local id of in's row 0 */
+    SpillRows out;               /* next frontier */
     unsigned long long out_cap;  /* states the next frontier holds in all (HBM part + host part) */
-    unsigned long long out_base; /* local id of out[0] */
+    unsigned long long out_base; /* local id of out's row 0 */
     uint64_t* table;             /* capacity entries of {fp, meta} */
     unsigned long long table_cap; /* entries: any multiple of VSR_BUCKET (not only powers of two: memory-bound configs size the seen-set to what is left) */
     uint64_t* trace;             /* per local id: make_trec(parent global id, candidate); may be null */
@@ -253,20 +248,6 @@ __device__ __forceinline__ int table_insert(uint64_t* table, unsigned long long 
     return table_insert_from(table, cap, h, p, fp, meta, probes, collisions);
 }
 
-/* TMA bulk store shared -> global of `bytes` (multiple of 16), issued by one lane; waits until the
-   shared source may be overwritten */
-__device__ __forceinline__ void bulk_store(void* gdst, const void* ssrc, uint32_t bytes) {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    const uint32_t s = (uint32_t)__cvta_generic_to_shared(ssrc);
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(s), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-}
-
-template <int NW> __device__ __forceinline__ uint32_t* out_state(const ExpandParams& P, unsigned long long i) {
-    return i < P.out_split ? P.out + i * NW : P.out_hi + (i - P.out_split) * NW;
-}
-
 /* ------------------------------------------------------------------ expand kernel */
 
 #ifdef VSR_QPS
@@ -403,15 +384,7 @@ template <class L, bool MULTI, bool COVER = false> struct Expander {
         if (base + n > P.out_cap) {
             if (lane == 0) atomicExch(&P.ctr->overflow, 1);
         } else {
-            if (lane == 0) {
-                if (base + n <= P.out_split) bulk_store(P.out + base * L::NW, S.stage, (uint32_t)(n * L::BYTES));
-                else if (base >= P.out_split) bulk_store(P.out_hi + (base - P.out_split) * L::NW, S.stage, (uint32_t)(n * L::BYTES));
-                else { /* the block of ids straddles the end of the HBM part */
-                    const int n1 = (int)(P.out_split - base);
-                    bulk_store(P.out + base * L::NW, S.stage, (uint32_t)(n1 * L::BYTES));
-                    bulk_store(P.out_hi, S.stage + n1 * L::NW, (uint32_t)((n - n1) * L::BYTES));
-                }
-            }
+            if (lane == 0) store_rows<L::NW>(P.out, base, S.stage, n);
             if (P.trace && lane < n && P.out_base + base + lane < P.trace_cap) P.trace[P.out_base + base + lane] = S.tstage[lane];
         }
         __syncwarp();
@@ -844,13 +817,13 @@ template <class L, bool MULTI, bool COVER = false> struct Expander {
 
     __device__ void run_round(unsigned long long first, int count) {
         /* coalesced load of `count` parent states into padded rows */
-        const uint32_t* src = P.in + first * L::NW;
-        if (first + count <= P.in_split) {
+        const uint32_t* src = P.in.hbm + first * L::NW;
+        if (P.in.in_hbm(first, count)) {
             for (int i = tid; i < count * L::NW; i += NS) B.par[(i / L::NW) * (L::NW + 1) + (i % L::NW)] = __ldg(src + i);
         } else { /* (part of) this round's parents are in the host part of the frontier */
             for (int i = tid; i < count * L::NW; i += NS) {
                 const unsigned long long st = first + i / L::NW;
-                const uint32_t* row = st < P.in_split ? P.in + st * L::NW : P.in_hi + (st - P.in_split) * L::NW;
+                const uint32_t* row = P.in.row<L::NW>(st);
                 B.par[(i / L::NW) * (L::NW + 1) + (i % L::NW)] = __ldg(row + i % L::NW);
             }
         }
@@ -965,10 +938,10 @@ template <class L, bool MULTI, bool COVER = false> __global__ void __launch_boun
             next_round = atomicAdd(&P.ctr->work_next, 1ull);
             /* pull the next round's parents into L2 while this round runs */
             const unsigned long long nx = next_round;
-            if (nx < nrounds && (nx + 1) * Smem::NR <= P.in_split) {
+            if (nx < nrounds && (nx + 1) * Smem::NR <= P.in.split) {
                 const unsigned long long nfirst = nx * Smem::NR;
                 const unsigned long long ncount = (P.n_in - nfirst) < (unsigned long long)Smem::NR ? (P.n_in - nfirst) : Smem::NR;
-                asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(P.in + nfirst * L::NW), "r"((uint32_t)(ncount * L::BYTES)) : "memory");
+                asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(P.in.hbm + nfirst * L::NW), "r"((uint32_t)(ncount * L::BYTES)) : "memory");
             }
         }
         const unsigned long long first = c * Smem::NR;
@@ -988,7 +961,7 @@ template <class L> __global__ void patch_ties_kernel(const ExpandParams P, const
     const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_out) return;
     uint32_t w[L::NW];
-    uint32_t* st = out_state<L::NW>(P, i);
+    uint32_t* st = P.out.row<L::NW>(i);
     for (int j = 0; j < L::NW; j++) w[j] = st[j];
     uint64_t fp = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
     if (fp == 0) fp = 1;
@@ -1071,11 +1044,11 @@ static __global__ void audit_table_kernel(const uint64_t* table, unsigned long l
     audit_add(&out->tagged_fp_sum, fs, false);
     audit_add(&out->tagged_fp_xor, fx, true);
 }
-template <class L> __global__ void audit_frontier_kernel(const ExpandParams P, unsigned long long n_states, AuditSums* out) {
+template <class L> __global__ void audit_frontier_kernel(const ExpandParams P, const SpillRows level, unsigned long long n_states, AuditSums* out) {
     unsigned long long found = 0, fs = 0, fx = 0, ws = 0, wx = 0;
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_states; i += (unsigned long long)gridDim.x * blockDim.x) {
         uint32_t w[L::NW];
-        const uint32_t* st = out_state<L::NW>(P, i);
+        const uint32_t* st = level.row<L::NW>(i);
         uint64_t hw = 0;
         for (int j = 0; j < L::NW; j++) {
             w[j] = st[j];
@@ -1122,9 +1095,8 @@ struct ReshardParams {
     const uint32_t* in;                /* n states of L::NW words */
     const uint64_t* in_trace;          /* their records in the old numbering */
     unsigned long long n;
-    uint32_t* out;                     /* frontier buffer 0: [0, out_split) in HBM, the rest at out_hi (spill) */
-    uint32_t* out_hi;
-    unsigned long long out_split, out_cap;
+    SpillRows out;                     /* frontier buffer 0 */
+    unsigned long long out_cap;
     uint64_t* trace;                   /* record of kept state j goes to trace[trace_base + j] (NULL: no trace) */
     unsigned long long trace_base, trace_cap;
     const uint64_t* table;             /* this rank's seen-set, already filled from every old file */
@@ -1164,7 +1136,7 @@ template <class L> __global__ void reshard_frontier_kernel(const ReshardParams P
         if (!mine) continue;
         const unsigned long long pos = base + __popc(m & ((1u << lane) - 1u));
         if (pos >= P.out_cap) continue; /* counted: the host reports the owned frontier's size */
-        uint32_t* dst = pos < P.out_split ? P.out + pos * L::NW : P.out_hi + (pos - P.out_split) * L::NW;
+        uint32_t* dst = P.out.row<L::NW>(pos);
         for (int j = 0; j < L::NW; j++) dst[j] = w[j];
         if (P.trace && P.trace_base + pos < P.trace_cap) P.trace[P.trace_base + pos] = remap_trec(P.remap, P.in_trace[i]);
     }

@@ -23,7 +23,7 @@ struct GpuOps {
     cudaError_t (*launch_simulate)(const SimParams&, int grid, cudaStream_t);
     /* the expand kernel's shape (ExpandCfg): warps per block, blocks per SM, scan passes per round, staging rows per warp */
     int warps, blocks, passes, stage_rows;
-    cudaError_t (*launch_audit)(const ExpandParams&, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t);
+    cudaError_t (*launch_audit)(const ExpandParams&, const SpillRows& level, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t);
     /* liveness pass (vsr_live.cuh): store a level's not-P states; one elimination sweep over store indices [first, first + n) */
     cudaError_t (*launch_live_collect)(const LiveParams&, int sms, cudaStream_t);
     cudaError_t (*launch_live_sweep)(const LiveParams&, int sms, cudaStream_t);
@@ -34,7 +34,8 @@ struct GpuOps {
 /* what a layout plug-in must have been compiled against: the version constant AND the shapes of the structs the kernels and the
    host exchange (a plug-in built from another revision of these headers must be rebuilt, never loaded) */
 inline int gpu_abi_value() {
-    return VSR_PLUGIN_ABI * 100000 + (int)((sizeof(ExpandParams) * 131 + sizeof(DevCounters) * 17 + sizeof(RecHdr) + VSR_BUCKET * 3) % 100000);
+    return VSR_PLUGIN_ABI * 100000 + (int)((sizeof(ExpandParams) * 131 + sizeof(LiveParams) * 61 + sizeof(ReshardParams) * 29 + sizeof(DevCounters) * 17 +
+                                            sizeof(SpillRows) * 5 + sizeof(RecHdr) + VSR_BUCKET * 3) % 100000);
 }
 
 template <class L> struct GpuThunks {
@@ -67,9 +68,9 @@ template <class L> struct GpuThunks {
         simulate_kernel<L><<<grid, 128, 0, st>>>(q);
         return cudaGetLastError();
     }
-    static cudaError_t launch_audit(const ExpandParams& p, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t st) {
+    static cudaError_t launch_audit(const ExpandParams& p, const SpillRows& level, unsigned long long n_states, AuditSums* out, int sms, cudaStream_t st) {
         audit_table_kernel<<<sms * 8, 256, 0, st>>>(p.table, p.table_cap, p.level, out);
-        if (n_states) audit_frontier_kernel<L><<<sms * 8, 256, 0, st>>>(p, n_states, out);
+        if (n_states) audit_frontier_kernel<L><<<sms * 8, 256, 0, st>>>(p, level, n_states, out);
         return cudaGetLastError();
     }
     static cudaError_t launch_live_collect(const LiveParams& q, int sms, cudaStream_t st) {

@@ -93,7 +93,7 @@ static bool load_layout_plugin(int R, int V, int K, LayoutPlugin* out, std::stri
     const std::string name = "libvsr_layout_" + std::to_string(R) + "_" + std::to_string(V) + "_" + std::to_string(K) + ".so";
     const std::string path = ldir + "/" + name;
     time_t newest = 0; /* of the sources the plug-in is made of */
-    for (const char* f : {"vsr_layout_plugin.cu", "vsr_gpu_thunks.cuh", "vsr_gpu.cuh", "vsr_thunks.h", "vsr_actions.h", "vsr_layout.h",
+    for (const char* f : {"vsr_layout_plugin.cu", "vsr_gpu_thunks.cuh", "vsr_gpu.cuh", "vsr_spill.cuh", "vsr_thunks.h", "vsr_actions.h", "vsr_layout.h",
                           "vsr_flat_conv.h", "vsr_model.h"})
         newest = std::max(newest, mtime_of(dir + "/csrc/" + f));
     std::string open_why;

@@ -42,10 +42,8 @@ uint64_t env_u64(const char* name) {
 LiveParams live_params(VsrEngine* e) {
     LiveParams q;
     memset(&q, 0, sizeof q);
-    q.words = e->live_words;
-    q.words_hi = e->live_words_host;
-    q.words_split = e->live_dev_cap;
-    q.cap = e->live_cap;
+    q.words = e->live_words.view();
+    q.cap = e->live_words.capacity();
     q.ids = e->live_ids;
     q.index = e->live_index;
     q.index_cap = e->live_index_cap;
@@ -94,17 +92,15 @@ int live_create(VsrEngine* e, char* err, size_t errcap) {
     dev = std::min(dev, cap);
     const uint64_t host = e->opts.frontier_host_capacity ? cap - dev : 0;
     if (!host) cap = dev = dev & ~31ull; /* the store ends with its HBM part (whole words of alive bits) */
-    if (dev && (cudaMallocAsync((void**)&e->live_words, dev * S, e->stream)) != cudaSuccess) {
+    if (e->live_words.alloc_hbm(dev, S, e->stream) != cudaSuccess) {
         cudaGetLastError();
         return fail(VSR_RC_TOO_LARGE, "liveness store: %llu states of %llu bytes do not fit in device memory", (unsigned long long)dev, (unsigned long long)S);
     }
-    if (host && (cudaHostAlloc((void**)&e->live_words_host, host * S, cudaHostAllocPortable | cudaHostAllocMapped)) != cudaSuccess) {
+    if (e->live_words.alloc_host(host) != cudaSuccess) {
         cudaGetLastError();
         return fail(VSR_RC_TOO_LARGE, "liveness store: %llu bytes of pinned host memory for its continuation (%llu states) cannot be allocated",
                     (unsigned long long)(host * S), (unsigned long long)host);
     }
-    e->live_cap = cap;
-    e->live_dev_cap = dev;
     e->live_bytes_hbm = e->live_index_cap * 16 + cap * 8 + abytes + dev * S;
     e->live_bytes_host = host * S;
     const int rc = live_reset(e);
@@ -117,15 +113,11 @@ void live_destroy(VsrEngine* e) {
     if (e->live_ids) cudaFreeAsync(e->live_ids, e->stream);
     if (e->live_alive) cudaFreeAsync(e->live_alive, e->stream);
     if (e->live_ctr) cudaFreeAsync(e->live_ctr, e->stream);
-    if (e->live_words) cudaFreeAsync(e->live_words, e->stream);
-    if (e->stream) cudaStreamSynchronize(e->stream);
-    if (e->live_words_host) cudaFreeHost(e->live_words_host);
+    e->live_words.release(e->stream);
     e->live_index = nullptr;
     e->live_ids = nullptr;
     e->live_alive = nullptr;
     e->live_ctr = nullptr;
-    e->live_words = nullptr;
-    e->live_words_host = nullptr;
 }
 
 int live_reset(VsrEngine* e) {
@@ -140,9 +132,7 @@ int live_reset(VsrEngine* e) {
 /* after vsr_engine_finish_level advanced: the level now current (depth e->level) goes into the store */
 int live_collect(VsrEngine* e) {
     LiveParams q = live_params(e);
-    q.in = e->frontier[e->cur];
-    q.in_hi = e->frontier_host[e->cur];
-    q.in_split = e->frontier_host_cap ? e->frontier_cap : ~0ull;
+    q.in = e->frontier[e->cur].view();
     q.n_in = e->n_cur;
     q.in_base = e->cur_base;
     std::vector<uint64_t>& off = e->live_level_off; /* off[d - 1] .. off[d]: depth d */
@@ -154,11 +144,11 @@ int live_collect(VsrEngine* e) {
     CK(cudaMemcpyAsync(&c, e->live_ctr, sizeof c, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     e->st.bytes_d2h += sizeof c;
-    off.push_back(std::min<uint64_t>(c.count, e->live_cap));
+    off.push_back(std::min<uint64_t>(c.count, e->live_words.capacity()));
     if (c.overflow) {
         snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (liveness %s): %llu not-P states at depth %d, the store holds %llu "
                  "(%llu in HBM; frontier_host_capacity > 0 lets it continue in host memory)", c.overflow == 1 ? "store" : "index",
-                 (unsigned long long)c.count, e->level, (unsigned long long)e->live_cap, (unsigned long long)e->live_dev_cap);
+                 (unsigned long long)c.count, e->level, (unsigned long long)e->live_words.capacity(), (unsigned long long)e->live_words.hbm_rows);
         return VSR_RC_TOO_LARGE;
     }
     if (c.error) {
@@ -189,12 +179,12 @@ int vsr_engine_liveness(VsrEngine* e, VsrLiveStats* out, uint32_t* cands_out, si
     const int nlev = (int)off.size() - 1;
     const uint64_t stored = live_stored(e);
     out->stored = stored;
-    out->capacity = e->live_cap;
+    out->capacity = e->live_words.capacity();
     out->bytes_hbm = e->live_bytes_hbm;
     out->bytes_host = e->live_bytes_host;
     out->violation_index = ~0ull;
     CK(cudaSetDevice(e->device));
-    CK(cudaMemsetAsync(e->live_alive, 0xFF, e->live_cap / 8, e->stream));
+    CK(cudaMemsetAsync(e->live_alive, 0xFF, e->live_words.capacity() / 8, e->stream));
     LiveParams q = live_params(e);
     LiveCtr c;
     memset(&c, 0, sizeof c);
@@ -259,8 +249,7 @@ int vsr_engine_liveness(VsrEngine* e, VsrLiveStats* out, uint32_t* cands_out, si
     CK(cudaMemcpy(&local_id, e->live_ids + vi, 8, cudaMemcpyDeviceToHost));
     if (walk_trace(e, local_id, prefix)) return VSR_RC_ERROR;
     uint32_t cur[VSR_MAX_STATE_BYTES / 4], nx[VSR_MAX_STATE_BYTES / 4], init[VSR_MAX_STATE_BYTES / 4];
-    if (vi < e->live_dev_cap) CK(cudaMemcpy(cur, e->live_words + vi * (S / 4), S, cudaMemcpyDeviceToHost));
-    else memcpy(cur, e->live_words_host + (vi - e->live_dev_cap) * (S / 4), S);
+    CK(e->live_words.to_host(vi, 1, cur));
     ops->init(init);
     auto key = [&](const uint32_t* w) {
         uint64_t fp = ops->fingerprint(w, run.use_view);

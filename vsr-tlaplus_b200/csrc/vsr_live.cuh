@@ -27,14 +27,12 @@ struct LiveCtr {
 };
 
 struct LiveParams {
-    /* collect: the level just finished, n_in states of L::NW words, [0, in_split) at in, the rest at in_hi (spill) */
-    const uint32_t* in;
-    const uint32_t* in_hi;
-    unsigned long long in_split, n_in, in_base;
-    /* the store: state s at words + s * NW for s < words_split, else in the host part */
-    uint32_t* words;
-    uint32_t* words_hi;
-    unsigned long long words_split, cap;
+    /* collect: the level just finished, n_in states of L::NW words */
+    SpillRows in;
+    unsigned long long n_in, in_base;
+    /* the store: state s is words' row s */
+    SpillRows words;
+    unsigned long long cap;
     unsigned long long* ids;      /* local (BFS) id of each stored state */
     uint64_t* index;
     unsigned long long index_cap;
@@ -47,10 +45,6 @@ struct LiveParams {
     unsigned long long first, n;  /* sweep: store indices [first, first + n) */
 };
 
-template <int NW> __device__ __forceinline__ uint32_t* live_state(const LiveParams& P, unsigned long long s) {
-    return s < P.words_split ? P.words + s * NW : P.words_hi + (s - P.words_split) * NW;
-}
-
 template <class L> __global__ void live_collect_kernel(const LiveParams P) {
     const unsigned lane = threadIdx.x & 31;
     const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
@@ -59,7 +53,7 @@ template <class L> __global__ void live_collect_kernel(const LiveParams P) {
         uint32_t w[L::NW];
         bool take = false;
         if (i < P.n_in) {
-            const uint32_t* st = i < P.in_split ? P.in + i * L::NW : P.in_hi + (i - P.in_split) * L::NW;
+            const uint32_t* st = P.in.row<L::NW>(i);
             for (int j = 0; j < L::NW; j++) w[j] = st[j];
             take = !Ops<L>::live_pred(P.run, w, P.hooks);
         }
@@ -73,7 +67,7 @@ template <class L> __global__ void live_collect_kernel(const LiveParams P) {
             atomicCAS(&P.ctr->overflow, 0, 1);
             continue;
         }
-        uint32_t* dst = live_state<L::NW>(P, s);
+        uint32_t* dst = P.words.row<L::NW>(s);
         for (int j = 0; j < L::NW; j++) dst[j] = w[j];
         P.ids[s] = P.in_base + i;
         uint64_t fp = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
@@ -110,7 +104,7 @@ template <class L> __global__ void live_sweep_kernel(const LiveParams P) {
     for (unsigned long long s = P.first + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < end; s += (unsigned long long)gridDim.x * blockDim.x) {
         if (!((P.alive[s >> 5] >> (s & 31)) & 1u)) continue;
         uint32_t w[L::NW], nx[L::NW];
-        const uint32_t* st = live_state<L::NW>(P, s);
+        const uint32_t* st = P.words.row<L::NW>(s);
         for (int j = 0; j < L::NW; j++) w[j] = st[j];
         uint64_t fps = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
         if (fps == 0) fps = 1;

@@ -46,8 +46,8 @@ struct ModelOps {
     int (*enabled_list)(const RunCfg*, const uint32_t*, uint32_t* out); /* register-mask form of the guards (the kernel's scan) */
     int (*property)(const RunCfg*, const uint32_t*, int live_hooks);   /* the liveness pass's state predicate (live_pred) */
 };
-/* bump when ModelOps / GpuOps / ExpandParams / SimParams change shape: a layout plug-in built against another value is rebuilt */
-#define VSR_PLUGIN_ABI 10
+/* bump when ModelOps / GpuOps / ExpandParams / LiveParams / ReshardParams / SimParams change shape: a layout plug-in built against another value is rebuilt */
+#define VSR_PLUGIN_ABI 11
 const ModelOps* find_model_ops(int R, int V, int K);
 const GpuOps* find_gpu_ops(int R, int V, int K); /* defined in vsr_gpu.cu */
 

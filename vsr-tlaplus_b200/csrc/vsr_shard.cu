@@ -145,7 +145,7 @@ uint64_t vsr_engine_default_inbox_records(const VsrEngine* e) {
        every peer has to map over CUDA IPC when the exchange is attached stays small: with 8 ranks mapping 7 inboxes of 2.7 GB
        (21 GB for the README constants) was most of the one-call API's 0.9 s around an 0.08 s BFS */
     const uint64_t w = (uint64_t)(e->world > 1 ? e->world : 1);
-    uint64_t cap = e->frontier_cap / (2 * w);
+    uint64_t cap = e->frontier[0].hbm_rows / (2 * w);
     if (cap > (1ull << 25) / w) cap = (1ull << 25) / w;
     if (cap < 4096) cap = 4096;
     return cap;
