@@ -85,9 +85,9 @@ __global__ void ckpt_reinsert_kernel(uint64_t* table, unsigned long long cap, co
 }
 
 /* old trace records renumbered into the new world's ids */
-__global__ void ckpt_remap_trace_kernel(const uint64_t* __restrict__ in, unsigned long long n, uint64_t* __restrict__ out, const GidRemap m) {
+__global__ void ckpt_remap_trace_kernel(const uint64_t* __restrict__ in, unsigned long long n, const SpillRows out, const GidRemap m) {
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
-        out[i] = remap_trec(m, in[i]);
+        *(uint64_t*)out.row<2>(i) = remap_trec(m, in[i]);
 }
 
 struct File {
@@ -152,10 +152,10 @@ int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals
     h.symmetry = e->m->run.symmetry; h.use_view = e->m->run.use_view; h.invariant = e->m->run.invariant;
     h.rank = e->rank; h.world = e->world;
     h.level = e->level;
-    h.keep_trace = e->trace ? 1 : 0;
+    h.keep_trace = e->trace_cap ? 1 : 0;
     h.n_cur = e->n_cur; h.cur_base = e->cur_base; h.next_base = e->next_base;
     h.n_entries = e->st.distinct; /* checked against what the compaction finds */
-    h.n_trace = e->trace ? std::min<uint64_t>(e->next_base, e->trace_cap) : 0;
+    h.n_trace = std::min<uint64_t>(e->next_base, e->trace_cap);
     h.records_sent = e->records_sent; h.records_received = e->records_received;
     const VsrStats& tot = totals ? *totals : e->st;
     if (fwrite(&h, sizeof h, 1, out.f) != 1 || fwrite(&e->st, sizeof(VsrStats), 1, out.f) != 1 || fwrite(&tot, sizeof(VsrStats), 1, out.f) != 1)
@@ -207,7 +207,7 @@ int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals
         host.resize(std::min(per, h.n_trace) * 8);
         for (uint64_t o = 0; o < h.n_trace; o += per) {
             const uint64_t k = std::min(per, h.n_trace - o);
-            CK(cudaMemcpy(host.data(), e->trace + o, k * 8, cudaMemcpyDeviceToHost));
+            CK(e->trace.to_host(o, k, host.data()));
             if (fwrite(host.data(), 8, k, out.f) != k) return io_error(e, "cannot write", tmp.c_str());
         }
         e->st.bytes_d2h += h.n_trace * 8;
@@ -245,12 +245,12 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
         snprintf(e->last_error, sizeof e->last_error, "recover: %s is rank %d of %d, this engine is rank %d of %d", path, h.rank, h.world, e->rank, e->world);
         return VSR_RC_CONFIG_ERROR;
     }
-    if (h.n_cur > e->frontier[0].capacity() || h.n_entries > e->table_cap - e->table_cap / 8 || (h.n_trace && e->trace && h.n_trace > e->trace_cap)) {
+    if (h.n_cur > e->frontier[0].capacity() || h.n_entries > e->table_cap - e->table_cap / 8 || (h.n_trace && e->trace_cap && h.n_trace > e->trace.capacity())) {
         snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (recover): the checkpoint holds %llu frontier states and %llu seen-set entries",
                  (unsigned long long)h.n_cur, (unsigned long long)h.n_entries);
         return VSR_RC_TOO_LARGE;
     }
-    if (e->trace && !h.n_trace && h.next_base) {
+    if (e->trace_cap && !h.n_trace && h.next_base) {
         snprintf(e->last_error, sizeof e->last_error, "recover: %s was written without trace records; continue it with keep_trace off (vsrmc -notrace)", path);
         return VSR_RC_CONFIG_ERROR;
     }
@@ -299,7 +299,7 @@ int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
         for (uint64_t o = 0; o < h.n_trace; o += per) {
             const uint64_t k = std::min(per, h.n_trace - o);
             if (fread(host.data(), 8, k, in.f) != k) return io_error(e, "truncated", path);
-            if (e->trace) CK(cudaMemcpy(e->trace + o, host.data(), k * 8, cudaMemcpyHostToDevice));
+            if (e->trace_cap) CK(e->trace.from_host(o, k, host.data()));
         }
     }
     /* the BFS position and this rank's statistics continue where they were; capacities are this engine's */
@@ -410,7 +410,7 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
         m.off[r] = T;
         T += h[r].next_base;
     }
-    if (e->trace && !h[0].keep_trace && T) {
+    if (e->trace_cap && !h[0].keep_trace && T) {
         snprintf(e->last_error, sizeof e->last_error, "recover: %s was written without trace records; continue it with keep_trace off (vsrmc -notrace)", files[0].c_str());
         return VSR_RC_CONFIG_ERROR;
     }
@@ -471,7 +471,7 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
     uint64_t kept = 0;
     {
         const uint64_t fcap_total = e->frontier[0].capacity();
-        const bool tr = e->trace && h[0].keep_trace;
+        const bool tr = e->trace_cap && h[0].keep_trace;
         const uint64_t per = std::max<uint64_t>(1, (std::min(IO_CHUNK, scratch_bytes) - 16) / (S + 8));
         const uint64_t tr_off = (per * S + 15) & ~15ull;
         ReshardParams q;
@@ -480,9 +480,9 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
         q.in_trace = tr ? (const uint64_t*)(scratch + tr_off) : nullptr;
         q.out = e->frontier[0].view();
         q.out_cap = fcap_total;
-        q.trace = tr ? e->trace : nullptr;
+        q.trace = e->trace.view();
         q.trace_base = cur_base;
-        q.trace_cap = e->trace_cap;
+        q.trace_cap = tr ? e->trace.capacity() : 0;
         q.table = e->table;
         q.table_cap = e->table_cap;
         q.fp_tab = e->fp_tab;
@@ -532,15 +532,15 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
                      "recover: the checkpoint's frontier and seen-set disagree: %llu frontier states rank %d owns are not in its seen-set at depth %d", counts[1], me, h[0].level);
             return VSR_RC_ERROR;
         }
-        if (tr && cur_base + kept > e->trace_cap) {
+        if (tr && cur_base + kept > e->trace.capacity()) {
             snprintf(e->last_error, sizeof e->last_error,
                      "capacity exceeded (recover): rank %d needs %llu trace records (%llu of the checkpoint's %llu, then %llu frontier copies), it holds %llu", me,
-                     (unsigned long long)(cur_base + kept), (unsigned long long)cur_base, (unsigned long long)T, (unsigned long long)kept, (unsigned long long)e->trace_cap);
+                     (unsigned long long)(cur_base + kept), (unsigned long long)cur_base, (unsigned long long)T, (unsigned long long)kept, (unsigned long long)e->trace.capacity());
             return VSR_RC_TOO_LARGE;
         }
     }
     /* 5. this rank's slice [lo, hi) of the old records, from whichever files hold it, renumbered on the device */
-    if (e->trace && h[0].keep_trace) {
+    if (e->trace_cap && h[0].keep_trace) {
         const uint64_t per = std::max<uint64_t>(1, std::min(IO_CHUNK, scratch_bytes) / 8);
         host.resize(per * 8);
         for (int r = 0; r < Wold; r++) {
@@ -554,7 +554,7 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
                 t_read += now_s() - t;
                 t = now_s();
                 CK(cudaMemcpyAsync(scratch, host.data(), k * 8, cudaMemcpyHostToDevice, e->stream));
-                ckpt_remap_trace_kernel<<<e->sms * 4, 256, 0, e->stream>>>((const uint64_t*)scratch, k, e->trace + (o - lo), m);
+                ckpt_remap_trace_kernel<<<e->sms * 4, 256, 0, e->stream>>>((const uint64_t*)scratch, k, e->trace.view().from(o - lo, 2), m);
                 CK(cudaGetLastError());
                 CK(cudaStreamSynchronize(e->stream));
                 t_trace += now_s() - t;

@@ -42,8 +42,9 @@ struct VsrEngine {
     uint64_t* table = nullptr;
     uint64_t table_cap = 0;
     vsr::SpillBuffer frontier[2];     /* states; each continues in pinned host memory with frontier_host_capacity */
-    uint64_t* trace = nullptr;
-    uint64_t trace_cap = 0;
+    vsr::SpillBuffer trace;           /* one 8-byte record per local id (rows of 2 words); in HBM, or all of it in pinned host
+                                         memory when HBM has no room and the run allows host memory (vsr_engine_create) */
+    uint64_t trace_cap = 0;           /* 0: the run keeps no trace */
     vsr::DevCounters* ctr = nullptr;
     uint8_t* ties = nullptr;
     uint64_t tie_cap = 0;

@@ -53,7 +53,7 @@ void fill_params(VsrEngine* e, ExpandParams& p) {
     p.out_base = e->next_base;
     p.table = e->table;
     p.table_cap = e->table_cap;
-    p.trace = e->trace;
+    p.trace = e->trace.view();
     p.trace_cap = e->trace_cap;
     p.ctr = e->ctr;
     p.ties = e->ties;
@@ -115,6 +115,31 @@ static int insert_records(VsrEngine* e, const void* recs, uint64_t n) {
     p.drain_n[0] = (unsigned)n;
     p.drain_total = n;
     return launch_expand(e, p);
+}
+
+/* The trace, allocated after the engine's other BFS buffers: in HBM when it fits there, so every run that fits keeps it
+   where it always was.  When it does not and the run allows host memory (frontier_host_capacity > 0, the liveness store's
+   rule), all of it goes to pinned host memory mapped into the device: each record is written once, by the flush that gives
+   its state an id, and read only to rebuild a counterexample, a checkpoint or a re-shard.  Test hook
+   VSR_B200_TRACE_HBM_RECORDS=k (such runs only): at most k records in HBM, the rest in host memory. */
+static cudaError_t trace_alloc(VsrEngine* e) {
+    const bool host_ok = e->opts.frontier_host_capacity > 0;
+    uint64_t hbm = e->trace_cap;
+    const char* k = getenv("VSR_B200_TRACE_HBM_RECORDS");
+    if (host_ok && k && k[0]) hbm = std::min<uint64_t>(hbm, strtoull(k, nullptr, 10));
+    cudaError_t ce = e->trace.alloc_hbm(hbm, 8, e->stream);
+    if (ce == cudaErrorMemoryAllocation && host_ok) {
+        cudaGetLastError();
+        e->trace.hbm = nullptr;
+        hbm = 0;
+        ce = e->trace.alloc_hbm(0, 8, e->stream);
+    }
+    if (ce != cudaSuccess) return ce;
+    if ((ce = e->trace.alloc_host(e->trace_cap - hbm)) != cudaSuccess) return ce;
+    if (e->trace.host_rows && e->opts.verbose)
+        fprintf(stderr, "trace: %llu of %llu records (%.2f GB) in pinned host memory\n", (unsigned long long)e->trace.host_rows,
+                (unsigned long long)e->trace_cap, e->trace.host_rows * 8e-9);
+    return cudaSuccess;
 }
 
 extern "C" {
@@ -191,12 +216,12 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
         if ((ce = e->frontier[i].alloc_hbm(fcap, S, e->stream)) != cudaSuccess) return bail("cudaMalloc(frontier)", ce);
     for (int i = 0; i < 2; i++) /* spill: each frontier buffer continues in pinned, device-mapped host memory */
         if ((ce = e->frontier[i].alloc_host(opts->frontier_host_capacity)) != cudaSuccess) return bail("cudaHostAlloc(frontier spill)", ce);
-    if (e->trace_cap && (ce = cudaMallocAsync((void**)&e->trace, e->trace_cap * 8, e->stream)) != cudaSuccess) return bail("cudaMalloc(trace)", ce);
     if ((ce = cudaMallocAsync((void**)&e->ctr, sizeof(LevelCounters), e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->ties, e->tie_cap * (size_t)e->g->tie_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->fp_tab, 8 * 256 * 8, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMallocAsync((void**)&e->init_rec, e->g->rec_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMemcpyAsync(e->fp_tab, fp64_table(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess) return bail("memcpy", ce);
+    if ((ce = trace_alloc(e)) != cudaSuccess) return bail(e->trace.host_rows ? "cudaHostAlloc(trace)" : "cudaMalloc(trace)", ce);
     e->st.table_capacity = tcap;
     e->st.frontier_capacity = e->frontier[0].capacity();
     e->st.bytes_table = tcap * 16;
@@ -218,7 +243,7 @@ void vsr_engine_destroy(VsrEngine* e) {
     if (!e) return;
     if (e->stream) cudaFreeAsync(e->table, e->stream); else cudaFree(e->table);
     for (SpillBuffer& f : e->frontier) f.release(e->stream);
-    if (e->stream) cudaFreeAsync(e->trace, e->stream); else cudaFree(e->trace);
+    e->trace.release(e->stream);
     if (e->stream) cudaFreeAsync(e->ctr, e->stream); else cudaFree(e->ctr);
     if (e->stream) cudaFreeAsync(e->ties, e->stream); else cudaFree(e->ties);
     if (e->stream) cudaFreeAsync(e->fp_tab, e->stream); else cudaFree(e->fp_tab);
@@ -479,9 +504,9 @@ int vsr_engine_read_frontier(VsrEngine* e, uint64_t first, uint64_t n, void* hos
 }
 
 int vsr_engine_trace_record(VsrEngine* e, uint64_t local_id, uint64_t* parent_out, uint32_t* cand_out) {
-    if (!e->trace || local_id >= e->trace_cap) return VSR_RC_ERROR;
+    if (local_id >= e->trace_cap) return VSR_RC_ERROR;
     uint64_t t = 0;
-    CK(cudaMemcpy(&t, e->trace + local_id, 8, cudaMemcpyDeviceToHost));
+    CK(e->trace.to_host(local_id, 1, &t));
     e->st.bytes_d2h += 8;
     *parent_out = (t >> 12) & GID_MASK;
     *cand_out = (uint32_t)(t & 0xFFF);

@@ -92,8 +92,8 @@ struct ExpandParams {
     unsigned long long out_base; /* local id of out's row 0 */
     uint64_t* table;             /* capacity entries of {fp, meta} */
     unsigned long long table_cap; /* entries: any multiple of VSR_BUCKET (not only powers of two: memory-bound configs size the seen-set to what is left) */
-    uint64_t* trace;             /* per local id: make_trec(parent global id, candidate); may be null */
-    unsigned long long trace_cap;
+    SpillRows trace;             /* per local id: make_trec(parent global id, candidate), rows of 2 words (HBM, or host memory) */
+    unsigned long long trace_cap; /* 0: no trace, never dereferenced */
     DevCounters* ctr;
     uint8_t* ties;               /* tie_cap entries of sizeof(TieRec) + L::BYTES */
     unsigned long long tie_cap;
@@ -370,6 +370,8 @@ template <class L, bool MULTI, bool COVER = false> struct Expander {
        ids, one TMA bulk store for the states, then move the remainder (< 32 states) down */
     static __device__ __noinline__ void flush(const ExpandParams& P, Stage& S, int lane, int n) {
         const int sn = SROWS == 32 ? n : S.sn; /* 32 rows: the whole batch, nothing to move down */
+        const SpillRows trace = P.trace; /* read before the atomic, whose latency hides these loads */
+        const unsigned long long trace_cap = P.trace_cap;
         unsigned long long base = 0;
         if (lane == 0) base = atomicAdd(&P.ctr->out_count, (unsigned long long)n);
         base = __shfl_sync(0xffffffffu, base, 0);
@@ -385,7 +387,7 @@ template <class L, bool MULTI, bool COVER = false> struct Expander {
             if (lane == 0) atomicExch(&P.ctr->overflow, 1);
         } else {
             if (lane == 0) store_rows<L::NW>(P.out, base, S.stage, n);
-            if (P.trace && lane < n && P.out_base + base + lane < P.trace_cap) P.trace[P.out_base + base + lane] = S.tstage[lane];
+            if (lane < n && P.out_base + base + lane < trace_cap) *(uint64_t*)trace.row<2>(P.out_base + base + lane) = S.tstage[lane];
         }
         __syncwarp();
         const int rest = sn - n;
@@ -979,9 +981,10 @@ template <class L> __global__ void patch_ties_kernel(const ExpandParams P, const
         if (t->auxkey < Ops<L>::aux_key(w)) {
             const uint32_t* tw = (const uint32_t*)((const uint8_t*)t + sizeof(TieRec));
             for (int j = 0; j < L::NW; j++) { w[j] = tw[j]; st[j] = tw[j]; }
-            if (P.trace && P.out_base + i < P.trace_cap) {
+            if (P.out_base + i < P.trace_cap) {
+                uint64_t* rec = (uint64_t*)P.trace.row<2>(P.out_base + i);
                 if (P.cover) { /* coverage follows the trace: the state now counts as found by the winner's action */
-                    const uint64_t was = P.trace[P.out_base + i];
+                    const uint64_t was = *rec;
                     const int a0 = (was >> 12) == ROOT_GID ? (int)VSR_ACT_INIT : Ops<L>::action_of((int)(was & 0xFFFu));
                     const int a1 = t->parent == ROOT_GID ? (int)VSR_ACT_INIT : Ops<L>::action_of((int)(t->cand & 0xFFFu));
                     if (a0 != a1) {
@@ -989,7 +992,7 @@ template <class L> __global__ void patch_ties_kernel(const ExpandParams P, const
                         atomicAdd(&P.cover[VSR_NUM_ACTIONS + a1], 1ull);
                     }
                 }
-                P.trace[P.out_base + i] = make_trec(t->parent, t->cand);
+                *rec = make_trec(t->parent, t->cand);
             }
         }
     }
@@ -1097,8 +1100,8 @@ struct ReshardParams {
     unsigned long long n;
     SpillRows out;                     /* frontier buffer 0 */
     unsigned long long out_cap;
-    uint64_t* trace;                   /* record of kept state j goes to trace[trace_base + j] (NULL: no trace) */
-    unsigned long long trace_base, trace_cap;
+    SpillRows trace;                   /* record of kept state j goes to row trace_base + j */
+    unsigned long long trace_base, trace_cap; /* trace_cap 0: no trace */
     const uint64_t* table;             /* this rank's seen-set, already filled from every old file */
     unsigned long long table_cap;
     const uint64_t* fp_tab;
@@ -1138,7 +1141,7 @@ template <class L> __global__ void reshard_frontier_kernel(const ReshardParams P
         if (pos >= P.out_cap) continue; /* counted: the host reports the owned frontier's size */
         uint32_t* dst = P.out.row<L::NW>(pos);
         for (int j = 0; j < L::NW; j++) dst[j] = w[j];
-        if (P.trace && P.trace_base + pos < P.trace_cap) P.trace[P.trace_base + pos] = remap_trec(P.remap, P.in_trace[i]);
+        if (P.trace_base + pos < P.trace_cap) *(uint64_t*)P.trace.row<2>(P.trace_base + pos) = remap_trec(P.remap, P.in_trace[i]);
     }
     for (int o = 16; o; o >>= 1) miss += __shfl_xor_sync(0xffffffffu, miss, o);
     if (lane == 0 && miss) atomicAdd(P.missing, miss);

@@ -241,7 +241,7 @@ int vsr_engine_liveness(VsrEngine* e, VsrLiveStats* out, uint32_t* cands_out, si
     const RunCfg& run = e->m->run;
     const int S = ops->bytes, hooks = e->m->live_hooks;
     std::vector<uint32_t> prefix, walk;
-    if (!e->trace || !cands_out) { /* no parent records kept: the verdict without a counterexample */
+    if (!e->trace_cap || !cands_out) { /* no parent records kept: the verdict without a counterexample */
         out->seconds_total = now_s() - t0;
         return VSR_RC_LIVENESS;
     }

@@ -501,7 +501,7 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
         tot.queue = q;
     }
     /* counterexample: follow (parent, candidate) records across ranks back to Init */
-    if (bad_gid != ~0ull && trace_cands && e->trace && opts->keep_trace) {
+    if (bad_gid != ~0ull && trace_cands && e->trace_cap && opts->keep_trace) {
         std::vector<uint32_t> cands;
         if ((rc = walk_trace(e, bad_gid, cands))) return rc;
         const size_t n = std::min(cands.size(), trace_cap);
@@ -613,7 +613,7 @@ int vsr_bfs(const VsrModel* m, const VsrRunOpts* opts, VsrStats* stats, void* tr
         VsrLiveStats ls;
         rc = vsr_engine_liveness(e, &ls, cands.data(), cands.size());
         if (rc == VSR_RC_LIVENESS) {
-            stats->trace_len = e->trace ? ls.trace_len + 1 : 0; /* > 0: a lasso was walked, replay it */
+            stats->trace_len = e->trace_cap ? ls.trace_len + 1 : 0; /* > 0: a lasso was walked, replay it */
             replay_counterexample(m, rc, cands.data(), ls.trace_len, stats, trace_out, trace_actions, trace_cap);
             stats->trace_loop = ls.trace_loop;
             stats->violation_level = ls.violation_level;

@@ -1,6 +1,6 @@
 /*
  * vsr_spill.cuh — a buffer of fixed-size rows that continues in pinned host memory, mapped into the device, once its part in
- * HBM is full (BASELINE configs[3]): the two frontier buffers and the liveness store's words.  Row i is at hbm + i * NW while
+ * HBM is full (BASELINE configs[3]): the two frontier buffers, the liveness store's words and the trace.  Row i is at hbm + i * NW while
  * i < split, and at host + (i - split) * NW after that.  Without a host part split = ~0, so "does this lie in HBM" is one
  * compare on the hot path.
  */
