@@ -60,7 +60,18 @@ typedef struct VsrModelInfo {
  * 150/151 and writes a message to err.
  * Constants: ReplicaCount 2..7, |Values| 1..7, StartViewOnTimerLimit 0..14, ClientCount 1, RestartEmptyLimit 0.  The
  * packed layouts of the reference's configurations and their neighbours are built in; any other combination is
- * compiled on first use into <library dir>/layouts/ (needs nvcc; VSR_B200_JIT=0 turns that into a 151). */
+ * compiled on first use into <library dir>/layouts/ (needs nvcc, 20 s to a minute; VSR_B200_JIT=0 turns that into a
+ * 151).  Only StartViewOnTimerLimit up to the value in this table builds; a larger one is a 151 naming the limit it
+ * exceeds (packed state over VSR_MAX_STATE_BYTES, or an action group over the expand kernel's 16-bit pool item):
+ * | ReplicaCount | \|Values\| = 1 | 2 | 3 | 4 | 5 | 6 | 7 |
+ * |---|---|---|---|---|---|---|---|
+ * | 2 | 14 | 14 | 14 | 14 | 14 | 14 | 12 |
+ * | 3 | 10 | 10 | 10 | 10 | 8 | 7 | 6 |
+ * | 4 | 5 | 5 | 5 | 5 | 5 | 4 | 4 |
+ * | 5 | 3 | 3 | 3 | 3 | 3 | 3 | 2 |
+ * | 6 | 2 | 2 | 2 | 2 | 2 | - | - |
+ * | 7 | 1 | 1 | 1 | - | - | - | - |
+ */
 int vsr_load(const char* cfg_path, const char* tla_path, VsrModel** out, char* err, size_t errcap);
 /* same, from the text of a cfg file */
 int vsr_load_cfg_text(const char* cfg_text, const char* tla_path, VsrModel** out, char* err, size_t errcap);

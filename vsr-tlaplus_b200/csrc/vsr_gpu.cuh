@@ -313,6 +313,13 @@ template <class L> struct ExpandCfg {
     static constexpr int PASSES = BLOCKS == 1 && sizeof(BlockSmemT<L, WARPS, 2>) <= SMEM_ONE ? 2 : 1;
 #endif
     typedef BlockSmemT<L, WARPS, PASSES> Smem;
+    /* the compile-time limits a layout must meet (Expander and vsr_layout_plugin.cu assert them; tests/harness/layout_table.cu
+       lists them for every layout) */
+    static constexpr int NS = WARPS * 32;
+    static constexpr int TBITS = NS <= 512 ? 9 : 10; /* pool item = thread (TBITS bits) | candidate offset in its group (the other 16 - TBITS) */
+    static constexpr bool POOL_ITEM_FITS = NS <= (1 << TBITS) && max_grp() < (1 << (16 - TBITS));
+    static constexpr bool POOL_COUNTERS_FIT = max_grp() * NS < 65536; /* 16-bit packed per-group counters of the scan */
+    static constexpr size_t SMEM_SM = 227 * 1024;    /* shared memory of one SM that a block may have */
 };
 
 /*
@@ -682,9 +689,10 @@ template <class L, bool MULTI, bool COVER = false> struct Expander {
     static constexpr int MW = moff(NG);       /* mask words per state */
     static constexpr int PW = (NG + 1) / 2;   /* packed 16-bit counters, two groups per word */
     static __host__ __device__ constexpr int max_grp() { int m = 0; for (int g = 0; g < NG; g++) m = O_::grp_size(g) > m ? O_::grp_size(g) : m; return m; }
-    static constexpr int TBITS = NS <= 512 ? 9 : 10; /* pool item = thread (TBITS bits) | candidate offset in its group (the other 16 - TBITS) */
-    static_assert(NS <= (1 << TBITS) && max_grp() < (1 << (16 - TBITS)), "pool item does not fit 16 bits");
-    static_assert(max_grp() * NS < 65536, "16-bit packed counters");
+    static constexpr int TBITS = ExpandCfg<L>::TBITS;
+    static_assert(NS == ExpandCfg<L>::NS && max_grp() == ExpandCfg<L>::max_grp(), "ExpandCfg's limits are about this kernel");
+    static_assert(ExpandCfg<L>::POOL_ITEM_FITS, "pool item does not fit 16 bits");
+    static_assert(ExpandCfg<L>::POOL_COUNTERS_FIT, "16-bit packed counters");
 
     template <int G> __device__ __forceinline__ void guards(const RegRow<L::NW>& st, uint32_t* m, uint32_t* pc) {
         O_::template enabled_group<G>(P.run, st, m + moff(G));

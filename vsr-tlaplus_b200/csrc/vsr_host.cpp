@@ -80,6 +80,33 @@ static bool try_open_plugin(const std::string& path, int R, int V, int K, Layout
     out->gpu = gpu();
     return true; /* stays loaded for the life of the process: models point into it */
 }
+/* A plug-in compile that stopped at one of the layout's compile-time limits (the vsr_limit_* classes of vsr_layout_plugin.cu,
+   whose numbers the compiler prints as "vsr_limit_state_bytes<BYTES, MAX> [with BYTES=288, MAX=256]"): one line naming each
+   limit it exceeds.  "" when the log shows none of them. */
+static std::string plugin_limit_message(const std::string& log) {
+    auto nums = [&](const char* cls, long long* a, long long* b) {
+        const size_t p = log.find(std::string(cls) + "<"), w = p == std::string::npos ? p : log.find("[with ", p);
+        if (w == std::string::npos) return false;
+        const char* s = log.c_str() + w;
+        const char* e1 = strchr(s, '=');
+        const char* e2 = e1 ? strchr(e1 + 1, '=') : nullptr;
+        if (!e1 || !e2) return false;
+        *a = strtoll(e1 + 1, nullptr, 10);
+        *b = strtoll(e2 + 1, nullptr, 10);
+        return true;
+    };
+    std::string out;
+    long long a, b;
+    auto add = [&](const std::string& m) { out += (out.empty() ? "" : "; ") + m; };
+    if (nums("vsr_limit_state_bytes", &a, &b))
+        add("the packed state would be " + std::to_string(a) + " bytes, more than " + std::to_string(b) + " (VSR_MAX_STATE_BYTES)");
+    if (nums("vsr_limit_smem_bytes", &a, &b))
+        add("the expand kernel's shared memory would be " + std::to_string(a) + " bytes, more than the " + std::to_string(b) + " of an SM");
+    if (nums("vsr_limit_pool_item", &a, &b))
+        add("an action group of " + std::to_string(a) + " bindings does not fit the expand kernel's 16-bit pool items (at most " +
+            std::to_string(b) + ")");
+    return out;
+}
 static bool load_layout_plugin(int R, int V, int K, LayoutPlugin* out, std::string& why) {
     std::lock_guard<std::mutex> guard(g_plugin_mu);
     const auto key = std::make_tuple(R, V, K);
@@ -125,8 +152,9 @@ static bool load_layout_plugin(int R, int V, int K, LayoutPlugin* out, std::stri
             std::stringstream ss;
             ss << lf.rdbuf();
             std::string t = ss.str();
+            const std::string limit = plugin_limit_message(t);
             if (t.size() > 600) t = t.substr(0, 600) + " ...";
-            open_why = "compiling it failed (" + nvcc + ", log " + log + "): " + t;
+            open_why = limit.empty() ? "compiling it failed (" + nvcc + ", log " + log + "): " + t : "the layout cannot be built: " + limit;
         }
     }
     if (fd >= 0) { flock(fd, LOCK_UN); close(fd); }
