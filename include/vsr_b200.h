@@ -157,10 +157,8 @@ typedef struct VsrRunOpts {
     /* checkpoint / recover: TLC's `-checkpoint <minutes>` and `-recover <dir>` (the reference's .gitignore:1 ignores TLC's
        states/ metadir, i.e. its users run with checkpoints).  checkpoint_path: file written at the first level boundary after
        checkpoint_seconds since the last one (0 = after every level; written to <path>.tmp and renamed, so an interrupted write
-       leaves the previous checkpoint intact); recover_path: continue the BFS from that file instead of Init.  With several
-       ranks every rank uses <path>.rank<r>.  A checkpoint written by another number of ranks (<path> of one rank, or
-       <path>.rank0 ... of several) is recovered too: every rank reads every old file and keeps the seen-set entries,
-       frontier states and trace records it owns.  NULL = off. */
+       leaves the previous checkpoint intact); recover_path: continue the BFS from the checkpoint at that base path instead of
+       Init (vsr_engine_recover).  With several ranks every rank writes <path>.rank<r>.  NULL = off. */
     const char* checkpoint_path;
     const char* recover_path;
     double checkpoint_seconds;
@@ -255,10 +253,14 @@ int vsr_engine_stats(const VsrEngine* e, VsrStats* out);
 int vsr_engine_lookup(VsrEngine* e, const void* state, int* level_out, int* owner_out);
 /* Checkpoint of this rank's shard at a level boundary (after vsr_engine_finish_level, before the next expansion): the
  * current frontier, every seen-set entry {fingerprint, meta}, the trace records and the run's statistics, to one file.
- * vsr_engine_recover loads it into a fresh (or reset) engine of the same model, rank and world (the primitive for one
- * rank's own file; vsr_bfs_sharded also re-shards a checkpoint of another world); the seen-set is re-inserted
- * entry by entry, so its capacity may differ from the one the checkpoint was written with.  `totals` (may be NULL) travels
- * with the file: vsr_bfs_sharded stores the job's running totals there.  150 = not a checkpoint of this model. */
+ * vsr_engine_recover loads this rank's share of the checkpoint at base path `path` into a fresh (or reset) engine of the
+ * same model: <path> when one rank wrote it, <path>.rank0 ... <path>.rank<W_old - 1> when W_old ranks did (both present:
+ * the one of this engine's world; 151 when neither is).  W_old and the engine's world may differ (1, 2, 4 or 8): the rank
+ * checks the header of every old file and reads the bulk of only those that hold its share — its own file in the same world,
+ * so a world-1 engine loads <path> as it always has.  The seen-set is re-inserted entry by entry, so its capacity may
+ * differ from the one the checkpoint was written with.  `totals` (may be NULL) travels with the file: vsr_bfs_sharded
+ * stores the job's running totals there.  150 = not a checkpoint of this model, or files that are not one checkpoint;
+ * 152 = this rank's share does not fit; 153 = a file cannot be opened. */
 int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals);
 int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out);
 /* forget everything explored (clears the seen-set, keeps the allocations): ready for seed_init again */

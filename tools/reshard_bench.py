@@ -2,14 +2,14 @@
 """reshard_bench.py — what recovering a checkpoint on another number of GPUs costs, on the shipped VSR.cfg.
 
 One GPU checkpoints the BFS at --depth (its INVARIANT dropped, so that the search goes on past depth 28), then the checkpoint
-is recovered twice: on one rank (the same-world path: each rank reads its own file) and on two ranks (the re-sharding
-path: each rank reads every old file and keeps its share).  Two GPUs are used when the machine has them, else two ranks
+is recovered twice through the one loader: on one rank (the same world: the rank reads its file and keeps every id
+where it was) and on two ranks (the world grows: each rank reads the one old file and keeps its share).  Two GPUs are used when the machine has them, else two ranks
 share device 0 through VSR_B200_MULTI_ONE_DEVICE; the JSON says which.  The two-rank run continues to the end of the
 search and its totals are compared with 1,173,992,337 distinct / 3,129,587,684 generated / depth 47.
 
 Prints one JSON line: the card's name and power limit (read in the same run), the checkpoint's size and how long writing
-it took, and per recovery its wall seconds.  For the re-sharding path the engine's own split is reported per rank
-(reading the files, seen-set insert, frontier kernel, trace) with the bytes each rank read.
+it took, and per recovery its wall seconds.  For the two-rank recovery the engine's own split is reported per rank
+(reading the files, seen-set insert, frontier kernel, trace) with the files and bytes each rank read.
 
     python tools/reshard_bench.py [--depth 30] [--trace] [--dir DIR]
 
@@ -89,7 +89,7 @@ def main():
         part = mc.check(max_depth=a.depth, checkpoint_path=ck, checkpoint_seconds=1e9, **one)
         out["checkpoint"] = {"rc": part.rc, "depth": part.depth, "distinct": part.distinct, "bytes": os.path.getsize(ck),
                              "frontier_states": part.level_sizes[-1], "bfs_and_write_seconds": time.time() - t0}
-        # the same-world path: one rank reads its own file, and stops at the boundary it recovered
+        # the same world: one rank reads its own file, and stops at the boundary it recovered
         t0 = time.time()
         same = mc.check(recover_path=ck, max_depth=a.depth, **one)
         out["recover_world1"] = {"rc": same.rc, "wall_seconds": time.time() - t0, "seconds_setup": same.seconds_setup,

@@ -537,7 +537,7 @@ class ModelChecker:
                  checkpoint_seconds: float = 0.0, coverage: bool = False) -> VsrRunOpts:
         """checkpoint_path / recover_path / checkpoint_seconds: TLC's -checkpoint / -recover (a file per rank at level
         boundaries; see include/vsr_b200.h VsrRunOpts).  recover_path may have been written by any number of GPUs: check()
-        and check_multi() re-shard it as they load it.  coverage: count TLC's action coverage (CheckResult.coverage)"""
+        and check_multi() load each rank's share of it.  coverage: count TLC's action coverage (CheckResult.coverage)"""
         o = VsrRunOpts()
         if coverage:
             o.cov = VsrCoverage()  # kept alive by the options object

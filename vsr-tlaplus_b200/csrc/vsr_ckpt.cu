@@ -220,147 +220,54 @@ int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals
     return 0;
 }
 
-int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
-    if (!e || !path) return VSR_RC_ERROR;
-    CK(cudaSetDevice(e->device));
-    File in;
-    in.f = fopen(path, "rb");
-    if (!in.f) return io_error(e, "cannot open", path);
-    CkptHeader h;
-    VsrStats mine, tot;
-    if (fread(&h, sizeof h, 1, in.f) != 1 || h.magic != CKPT_MAGIC || h.version != 1 || h.header_bytes != sizeof h || h.stats_bytes != sizeof(VsrStats)) {
-        snprintf(e->last_error, sizeof e->last_error, "recover: %s is not a checkpoint of this build", path);
-        return VSR_RC_SPEC_ERROR;
-    }
-    if (fread(&mine, sizeof mine, 1, in.f) != 1 || fread(&tot, sizeof tot, 1, in.f) != 1) return io_error(e, "truncated", path);
-    const uint64_t S = (uint64_t)e->g->bytes;
-    if (h.state_bytes != S || h.R != e->g->R || h.V != e->g->V || h.K != e->g->K || h.symmetry != e->m->run.symmetry || h.use_view != e->m->run.use_view ||
-        h.invariant != e->m->run.invariant) {
-        snprintf(e->last_error, sizeof e->last_error,
-                 "recover: %s was written for ReplicaCount=%d |Values|=%d StartViewOnTimerLimit=%d symmetry=%d view=%d invariants=%d: not this model", path,
-                 h.R, h.V, h.K - 1, h.symmetry, h.use_view, h.invariant);
-        return VSR_RC_SPEC_ERROR;
-    }
-    if (h.rank != e->rank || h.world != e->world) {
-        snprintf(e->last_error, sizeof e->last_error, "recover: %s is rank %d of %d, this engine is rank %d of %d", path, h.rank, h.world, e->rank, e->world);
-        return VSR_RC_CONFIG_ERROR;
-    }
-    if (h.n_cur > e->frontier[0].capacity() || h.n_entries > e->table_cap - e->table_cap / 8 || (h.n_trace && e->trace_cap && h.n_trace > e->trace.capacity())) {
-        snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (recover): the checkpoint holds %llu frontier states and %llu seen-set entries",
-                 (unsigned long long)h.n_cur, (unsigned long long)h.n_entries);
-        return VSR_RC_TOO_LARGE;
-    }
-    if (e->trace_cap && !h.n_trace && h.next_base) {
-        snprintf(e->last_error, sizeof e->last_error, "recover: %s was written without trace records; continue it with keep_trace off (vsrmc -notrace)", path);
-        return VSR_RC_CONFIG_ERROR;
-    }
-    int rc = vsr_engine_reset(e);
-    if (rc) return rc;
-    e->touched = true; /* from here on a failure leaves part of the checkpoint in the engine */
-    CK(cudaStreamSynchronize(e->stream));
-    std::vector<uint8_t> host;
-    /* 1. the frontier, into buffer 0 */
-    e->cur = 0;
-    {
-        const uint64_t per = std::max<uint64_t>(1, IO_CHUNK / S);
-        host.resize(per * S);
-        for (uint64_t first = 0; first < h.n_cur; first += per) {
-            const uint64_t n = std::min(per, h.n_cur - first);
-            if (fread(host.data(), S, n, in.f) != n) return io_error(e, "truncated", path);
-            CK(e->frontier[0].from_host(first, n, host.data()));
-        }
-    }
-    /* 2. the seen-set, re-inserted through the idle frontier buffer */
-    {
-        uint64_t* scratch = (uint64_t*)e->frontier[1].hbm;
-        const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>(IO_CHUNK / 16, e->frontier[1].hbm_rows * S / 16));
-        unsigned long long* dbad = &e->ctr->work_next;
-        CK(cudaMemsetAsync(dbad, 0, 8, e->stream));
-        host.resize(per * 16);
-        for (uint64_t o = 0; o < h.n_entries; o += per) {
-            const uint64_t k = std::min(per, h.n_entries - o);
-            if (fread(host.data(), 16, k, in.f) != k) return io_error(e, "truncated", path);
-            CK(cudaMemcpyAsync(scratch, host.data(), k * 16, cudaMemcpyHostToDevice, e->stream));
-            ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, scratch, k, 64, 0, dbad, nullptr);
-            CK(cudaGetLastError());
-            CK(cudaStreamSynchronize(e->stream)); /* `host` is reused by the next round */
-        }
-        unsigned long long bad = 0;
-        CK(cudaMemcpy(&bad, dbad, 8, cudaMemcpyDeviceToHost));
-        if (bad) {
-            snprintf(e->last_error, sizeof e->last_error, "recover: %llu seen-set entries of %s could not be inserted as new (corrupt file?)", bad, path);
-            return VSR_RC_ERROR;
-        }
-    }
-    /* 3. the trace records */
-    if (h.n_trace) {
-        const uint64_t per = IO_CHUNK / 8;
-        host.resize(std::min(per, h.n_trace) * 8);
-        for (uint64_t o = 0; o < h.n_trace; o += per) {
-            const uint64_t k = std::min(per, h.n_trace - o);
-            if (fread(host.data(), 8, k, in.f) != k) return io_error(e, "truncated", path);
-            if (e->trace_cap) CK(e->trace.from_host(o, k, host.data()));
-        }
-    }
-    /* the BFS position and this rank's statistics continue where they were; capacities are this engine's */
-    const uint64_t tc = e->st.table_capacity, fc = e->st.frontier_capacity, bt = e->st.bytes_table, bf = e->st.bytes_frontier;
-    e->st = mine;
-    e->st.table_capacity = tc; e->st.frontier_capacity = fc; e->st.bytes_table = bt; e->st.bytes_frontier = bf;
-    e->st.bytes_h2d += h.n_cur * S + h.n_entries * 16 + h.n_trace * 8;
-    e->n_cur = h.n_cur; e->cur_base = h.cur_base; e->next_base = h.next_base;
-    e->level = h.level;
-    e->level_open = false;
-    if (e->opts.collect_levels) e->collected.resize(h.level); /* depths up to the checkpoint's were collected by another run: empty */
-    e->records_sent = h.records_sent; e->records_received = h.records_received;
-    if (totals_out) *totals_out = tot;
-    return 0;
-}
-
 } /* extern "C" */
 
-/* ------------------------------------------------------------------ recovery on another number of ranks
- * Ownership is a pure function of the fingerprint, so the old files already hold everything a new rank needs: every rank of
- * the recovering world reads EVERY old file and keeps its own share — no exchange between the ranks, no peer memory.
- *   seen-set  the entries it owns (ckpt_reinsert_kernel's owner filter)
- *   frontier  the states it owns (reshard_frontier_kernel: the BFS's fingerprint and owner rule), appended to buffer 0, each
- *             with a copy of its old trace record; every kept state must be in the seen-set just filled
- *   trace     one global order of the old records, F(r, l) = off[r] + l, cut into W_new slices (GidRemap); the rank loads
- *             its slice, renumbering every parent, and its frontier's records follow the slice
- * A checkpoint of W_old ranks is read W_new times over in all.  The job's totals travel unchanged (the violation id renumbered);
- * of this rank's own counters only `distinct` (= entries it inserted, which its next checkpoint checks) carries over: the
- * per-rank work counters (generated, probes, launches, records sent / received, ...) start at 0. */
+/* ------------------------------------------------------------------ recovery on any number of ranks
+ * A checkpoint of W_old ranks continues on W_new ranks, both powers of two.  The owner is the top bits of fp x C
+ * (owner_of), so the owners nest, and each new rank reads the bulk sections of its source files only:
+ *   W_old = k W_new (k >= 1)  new rank r owns exactly what old ranks r k ... r k + k - 1 owned: it takes their seen-set
+ *                             entries and frontiers whole, and their trace records stay where they were (k = 1: same ids)
+ *   W_new = s W_old (s > 1)   new rank r's share lies in old file r / s: the entries and frontier states it owns
+ *                             (reshard_frontier_kernel: the BFS's fingerprint and owner rule), and slice r % s of the file's
+ *                             trace records, its frontier's records copied after the slice
+ * Every rank still checks the headers, statistics and job totals of every old file, so that all the files are one
+ * checkpoint.  Every stored global id is renumbered with one GidRemap (vsr_gpu.cuh).  The job's totals travel unchanged
+ * (the violation id renumbered).  In the same world the rank continues its file's counters; in another world only
+ * `distinct` (= entries it inserted, which its next checkpoint checks) carries over, the work counters start at 0. */
+namespace {
 
-int ckpt_old_files(VsrEngine* e, const char* base, std::vector<std::string>& files) {
-    files.clear();
+/* <base> when one rank wrote it, <base>.rank0 ... <base>.rank(W_old - 1) when several did (W_old from <base>.rank0's
+   header).  Both: the one of this world, 151 when neither is.  Anything else is the one file the loader names. */
+int old_files(VsrEngine* e, const char* base, std::vector<std::string>& files) {
     const std::string P = base, P0 = P + ".rank0";
     CkptHeader h1, h0;
-    const int k1 = peek_header(P, h1), k0 = peek_header(P0, h0);
-    const int W = e->world;
-    const int k = W > 1 ? k0 : k1;
-    const CkptHeader& h = W > 1 ? h0 : h1;
-    if (k == 0 || (k == 1 && h.world == W)) return 0; /* this world's own files (or not a checkpoint: vsr_engine_recover says so) */
-    const bool one = k1 == 1 && h1.world == 1;       /* what a one-rank writer leaves */
-    if (one && k0 == 1) {
+    const int k1 = peek_header(P, h1), k0 = peek_header(P0, h0), W = e->world;
+    const bool one = k1 == 1 && h1.world == 1;
+    if (one && k0 == 1 && W != 1 && W != h0.world) {
         snprintf(e->last_error, sizeof e->last_error, "recover: both %s (1 rank) and %s (%d ranks) exist and neither was written by %d ranks: remove one",
                  P.c_str(), P0.c_str(), h0.world, W);
         return VSR_RC_CONFIG_ERROR;
     }
-    if (k0 == 1) {
-        if (h0.world < 1 || h0.world > MAX_WORLD) {
+    if (k0 == 1 && !(one && W == 1)) {
+        if (h0.world < 1 || h0.world > MAX_WORLD || (h0.world & (h0.world - 1))) {
             snprintf(e->last_error, sizeof e->last_error, "recover: %s claims a world of %d ranks", P0.c_str(), h0.world);
             return VSR_RC_SPEC_ERROR;
         }
         for (int r = 0; r < h0.world; r++) files.push_back(P + ".rank" + std::to_string(r));
-    } else if (one || k1 == 0) {
-        files.push_back(P); /* k1 == 0 (several ranks): not a checkpoint, which the loader reports by name */
-    } else if (k0 == 0) {
-        files.push_back(P0);
+    } else {
+        files.push_back(k1 == -1 && (k0 == 0 || W > 1) ? P0 : P); /* not a checkpoint, or missing: the loader says which */
     }
-    return 0; /* no file at all: vsr_engine_recover reports this world's missing file */
+    return 0;
 }
 
-int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, VsrStats* totals_out) {
+} // namespace
+
+extern "C" int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
+    if (!e || !path) return VSR_RC_ERROR;
     CK(cudaSetDevice(e->device));
+    std::vector<std::string> files;
+    int rc = old_files(e, path, files);
+    if (rc) return rc;
     const int Wold = (int)files.size(), W = e->world, me = e->rank;
     const uint64_t S = (uint64_t)e->g->bytes;
     const double t_start = now_s();
@@ -368,56 +275,81 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
     uint64_t bytes_read = 0;
     std::vector<File> in(Wold);
     std::vector<CkptHeader> h(Wold);
-    VsrStats tot, mine, other;
-    /* 1. every old file: a checkpoint of this model, rank r of Wold, of the same level and job */
-    for (int r = 0; r < Wold; r++) {
-        const char* path = files[r].c_str();
-        in[r].f = fopen(path, "rb");
-        if (!in[r].f) return io_error(e, "cannot open", path);
-        if (fread(&h[r], sizeof h[r], 1, in[r].f) != 1 || !header_ok(h[r])) {
-            snprintf(e->last_error, sizeof e->last_error, "recover: %s is not a checkpoint of this build", path);
+    VsrStats tot{}, mine{}, st, st_tot;
+    /* 1. every old file: a checkpoint of this build and model, rank q of Wold, of the same level and job */
+    for (int q = 0; q < Wold; q++) {
+        const char* f = files[q].c_str();
+        in[q].f = fopen(f, "rb");
+        if (!in[q].f) return io_error(e, "cannot open", f);
+        if (fread(&h[q], sizeof h[q], 1, in[q].f) != 1 || !header_ok(h[q])) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s is not a checkpoint of this build", f);
             return VSR_RC_SPEC_ERROR;
         }
-        if (fread(&mine, sizeof mine, 1, in[r].f) != 1 || fread(r ? &other : &tot, sizeof tot, 1, in[r].f) != 1) return io_error(e, "truncated", path);
-        const CkptHeader& x = h[r];
+        if (fread(&st, sizeof st, 1, in[q].f) != 1 || fread(&st_tot, sizeof st_tot, 1, in[q].f) != 1) return io_error(e, "truncated", f);
+        const CkptHeader& x = h[q];
         if (x.state_bytes != S || x.R != e->g->R || x.V != e->g->V || x.K != e->g->K || x.symmetry != e->m->run.symmetry || x.use_view != e->m->run.use_view ||
             x.invariant != e->m->run.invariant) {
             snprintf(e->last_error, sizeof e->last_error,
-                     "recover: %s was written for ReplicaCount=%d |Values|=%d StartViewOnTimerLimit=%d symmetry=%d view=%d invariants=%d: not this model", path,
+                     "recover: %s was written for ReplicaCount=%d |Values|=%d StartViewOnTimerLimit=%d symmetry=%d view=%d invariants=%d: not this model", f,
                      x.R, x.V, x.K - 1, x.symmetry, x.use_view, x.invariant);
             return VSR_RC_SPEC_ERROR;
         }
-        if (x.world != Wold || x.rank != r) {
-            snprintf(e->last_error, sizeof e->last_error, "recover: %s is rank %d of %d, expected rank %d of %d", path, x.rank, x.world, r, Wold);
+        if (x.world != Wold || x.rank != q) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s is rank %d of %d, expected rank %d of %d", f, x.rank, x.world, q, Wold);
             return VSR_RC_SPEC_ERROR;
         }
-        if (r && (x.level != h[0].level || x.keep_trace != h[0].keep_trace || memcmp(&other, &tot, sizeof tot) != 0)) {
-            snprintf(e->last_error, sizeof e->last_error, "recover: %s is not of the same checkpoint as %s (level, trace or job totals differ)", path, files[0].c_str());
+        if (q && (x.level != h[0].level || x.keep_trace != h[0].keep_trace || memcmp(&st_tot, &tot, sizeof tot) != 0)) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s is not of the same checkpoint as %s (level, trace or job totals differ)", f, files[0].c_str());
+            return VSR_RC_SPEC_ERROR;
+        }
+        if (x.next_base != x.cur_base + x.n_cur) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s holds a frontier of %llu states at local id %llu, its next id is %llu", f,
+                     (unsigned long long)x.n_cur, (unsigned long long)x.cur_base, (unsigned long long)x.next_base);
             return VSR_RC_SPEC_ERROR;
         }
         if (x.n_trace && x.n_trace != x.next_base) {
-            snprintf(e->last_error, sizeof e->last_error, "recover: %s holds %llu of its %llu trace records", path, (unsigned long long)x.n_trace,
+            snprintf(e->last_error, sizeof e->last_error, "recover: %s holds %llu of its %llu trace records", f, (unsigned long long)x.n_trace,
                      (unsigned long long)x.next_base);
             return VSR_RC_SPEC_ERROR;
         }
+        if (q == 0) tot = st_tot;
+        if (q == me) mine = st;
     }
-    /* 2. the id mapping: old records in file order, cut into W slices */
+    /* 2. the source files [src, src + nsrc) and the id mapping */
+    const bool grow = W > Wold;
+    const int k = grow ? 1 : Wold / W, s = grow ? W / Wold : 1;
+    const int src = grow ? me / s : me * k, nsrc = grow ? 1 : k;
     GidRemap m;
     memset(&m, 0, sizeof m);
     m.old_world = Wold;
     uint64_t T = 0;
-    for (int r = 0; r < Wold; r++) {
-        m.off[r] = T;
-        T += h[r].next_base;
+    for (int g = 0; g < Wold; g += k) {
+        uint64_t hist = 0, front = 0;
+        for (int q = g; q < g + k; q++) front += h[q].cur_base;
+        for (int q = g; q < g + k; q++) {
+            T += h[q].next_base;
+            m.to[q] = grow ? q * s : g / k;
+            m.slice[q] = grow ? std::max<uint64_t>(1, (h[q].next_base + s - 1) / s) : REMAP_ALL;
+            m.cut[q] = grow ? REMAP_ALL : h[q].cur_base;
+            m.hist[q] = grow ? 0 : hist;
+            m.front[q] = grow ? 0 : front;
+            hist += h[q].cur_base;
+            front += h[q].n_cur;
+        }
     }
     if (e->trace_cap && !h[0].keep_trace && T) {
         snprintf(e->last_error, sizeof e->last_error, "recover: %s was written without trace records; continue it with keep_trace off (vsrmc -notrace)", files[0].c_str());
         return VSR_RC_CONFIG_ERROR;
     }
-    m.slice = std::max<uint64_t>(1, (T + W - 1) / W);
-    const uint64_t lo = std::min<uint64_t>(T, (uint64_t)me * m.slice), hi = std::min<uint64_t>(T, lo + m.slice);
-    const uint64_t cur_base = hi - lo;
-    int rc = vsr_engine_reset(e);
+    const bool tr = e->trace_cap && h[0].keep_trace;
+    /* this rank's old ids in each source file: grow, its slice of file src; else all of them */
+    uint64_t lo = 0, hi = h[src].next_base;
+    if (grow) {
+        lo = std::min<uint64_t>(hi, (uint64_t)(me % s) * m.slice[src]);
+        hi = std::min<uint64_t>(hi, lo + m.slice[src]);
+    }
+    const uint64_t cur_base = grow ? hi - lo : m.front[src]; /* the group's histories, then its frontiers */
+    rc = vsr_engine_reset(e);
     if (rc) return rc;
     e->touched = true; /* from here on a failure leaves part of the checkpoint in the engine */
     CK(cudaStreamSynchronize(e->stream));
@@ -431,58 +363,60 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
     const uint64_t limit = e->table_cap - e->table_cap / 8;
     unsigned long long counts[2] = {0, 0}; /* entries not new, entries owned */
     uint64_t n_entries = 0;
-    for (int r = 0; r < Wold; r++) n_entries += h[r].n_entries;
+    for (int q = src; q < src + nsrc; q++) n_entries += h[q].n_entries;
     {
         const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>({IO_CHUNK / 16, scratch_bytes / 16, e->table_cap / 16}));
         CK(cudaMemsetAsync(d0, 0, 16, e->stream));
         host.resize(per * 16);
-        for (int r = 0; r < Wold; r++) {
-            if ((rc = seek(e, in[r], entries_at(h[r]), files[r].c_str()))) return rc;
-            for (uint64_t o = 0; o < h[r].n_entries; o += per) {
-                const uint64_t k = std::min(per, h[r].n_entries - o);
+        for (int q = src; q < src + nsrc; q++) {
+            if ((rc = seek(e, in[q], entries_at(h[q]), files[q].c_str()))) return rc;
+            for (uint64_t o = 0; o < h[q].n_entries; o += per) {
+                const uint64_t n = std::min(per, h[q].n_entries - o);
                 double t = now_s();
-                if (fread(host.data(), 16, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                if (fread(host.data(), 16, n, in[q].f) != n) return io_error(e, "truncated", files[q].c_str());
                 t_read += now_s() - t;
                 t = now_s();
-                CK(cudaMemcpyAsync(scratch, host.data(), k * 16, cudaMemcpyHostToDevice, e->stream));
-                ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, (const uint64_t*)scratch, k, e->owner_shift, me, d0, d1);
+                CK(cudaMemcpyAsync(scratch, host.data(), n * 16, cudaMemcpyHostToDevice, e->stream));
+                ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, (const uint64_t*)scratch, n, e->owner_shift, me, d0, d1);
                 CK(cudaGetLastError());
                 CK(cudaMemcpyAsync(counts, d0, 16, cudaMemcpyDeviceToHost, e->stream));
                 CK(cudaStreamSynchronize(e->stream)); /* `host` is reused by the next round */
                 t_insert += now_s() - t;
-                bytes_read += k * 16;
-                e->st.bytes_h2d += k * 16;
+                bytes_read += n * 16;
                 if (counts[1] > limit) {
                     snprintf(e->last_error, sizeof e->last_error,
-                             "capacity exceeded (recover): rank %d of %d owns more than %llu of the checkpoint's %llu seen-set entries: 7/8 of its %llu slots",
-                             me, W, (unsigned long long)limit, (unsigned long long)n_entries, (unsigned long long)e->table_cap);
+                             "capacity exceeded (recover): rank %d of %d owns more than %llu of the checkpoint's seen-set entries: 7/8 of its %llu slots", me, W,
+                             (unsigned long long)limit, (unsigned long long)e->table_cap);
                     return VSR_RC_TOO_LARGE;
                 }
             }
         }
-        if (counts[0]) {
-            snprintf(e->last_error, sizeof e->last_error, "recover: %llu seen-set entries of %s and the other ranks' files could not be inserted as new (corrupt file?)", counts[0],
-                     files[0].c_str());
+        /* shrinking or the same world: every entry of a source file is this rank's */
+        const unsigned long long bad = counts[0] + (grow ? 0 : n_entries - counts[1]);
+        if (bad) {
+            snprintf(e->last_error, sizeof e->last_error, "recover: %llu seen-set entries of %s could not be inserted as new (corrupt file?)", bad,
+                     files[src].c_str());
             return VSR_RC_ERROR;
         }
     }
     const uint64_t owned = counts[1];
-    /* 4. the frontier states this rank owns, into buffer 0, with their trace records after this rank's slice */
-    uint64_t kept = 0;
+    /* 4. the frontier states, into buffer 0: shrinking or the same world, each source file's whole frontier in file order;
+       growing, the states this rank owns, with their trace records after its slice */
+    uint64_t kept = 0, launches = 0;
     {
         const uint64_t fcap_total = e->frontier[0].capacity();
-        const bool tr = e->trace_cap && h[0].keep_trace;
+        const bool copy = grow && tr;
         const uint64_t per = std::max<uint64_t>(1, (std::min(IO_CHUNK, scratch_bytes) - 16) / (S + 8));
         const uint64_t tr_off = (per * S + 15) & ~15ull;
         ReshardParams q;
         memset(&q, 0, sizeof q);
         q.in = (const uint32_t*)scratch;
-        q.in_trace = tr ? (const uint64_t*)(scratch + tr_off) : nullptr;
+        q.in_trace = copy ? (const uint64_t*)(scratch + tr_off) : nullptr;
         q.out = e->frontier[0].view();
         q.out_cap = fcap_total;
         q.trace = e->trace.view();
         q.trace_base = cur_base;
-        q.trace_cap = tr ? e->trace.capacity() : 0;
+        q.trace_cap = copy ? e->trace.capacity() : 0;
         q.table = e->table;
         q.table_cap = e->table_cap;
         q.fp_tab = e->fp_tab;
@@ -490,38 +424,40 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
         q.rank = me;
         q.owner_shift = e->owner_shift;
         q.level = h[0].level;
+        q.place = !grow;
         q.remap = m;
         q.kept = d0;
         q.missing = d1;
         CK(cudaMemsetAsync(d0, 0, 16, e->stream));
         host.resize(per * (S + 8));
         uint64_t* host_tr = (uint64_t*)(host.data() + per * S);
-        for (int r = 0; r < Wold; r++) {
+        for (int r = src; r < src + nsrc; r++) {
             const uint64_t n_cur = h[r].n_cur;
             for (uint64_t o = 0; o < n_cur; o += per) {
-                const uint64_t k = std::min(per, n_cur - o);
+                const uint64_t n = std::min(per, n_cur - o);
                 double t = now_s();
                 if ((rc = seek(e, in[r], SECTIONS + o * S, files[r].c_str()))) return rc;
-                if (fread(host.data(), S, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
-                if (tr) {
+                if (fread(host.data(), S, n, in[r].f) != n) return io_error(e, "truncated", files[r].c_str());
+                if (copy) {
                     if ((rc = seek(e, in[r], trace_at(h[r]) + (h[r].cur_base + o) * 8, files[r].c_str()))) return rc;
-                    if (fread(host_tr, 8, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                    if (fread(host_tr, 8, n, in[r].f) != n) return io_error(e, "truncated", files[r].c_str());
                 }
                 t_read += now_s() - t;
                 t = now_s();
-                CK(cudaMemcpyAsync(scratch, host.data(), k * S, cudaMemcpyHostToDevice, e->stream));
-                if (tr) CK(cudaMemcpyAsync(scratch + tr_off, host_tr, k * 8, cudaMemcpyHostToDevice, e->stream));
-                q.n = k;
+                CK(cudaMemcpyAsync(scratch, host.data(), n * S, cudaMemcpyHostToDevice, e->stream));
+                if (copy) CK(cudaMemcpyAsync(scratch + tr_off, host_tr, n * 8, cudaMemcpyHostToDevice, e->stream));
+                q.n = n;
+                q.out_first = kept + o;
                 CK(e->g->launch_reshard_frontier(q, e->sms, e->stream));
                 CK(cudaStreamSynchronize(e->stream));
-                e->st.kernel_launches++;
+                launches++;
                 t_frontier += now_s() - t;
-                bytes_read += k * (S + (tr ? 8 : 0));
-                e->st.bytes_h2d += k * (S + (tr ? 8 : 0));
+                bytes_read += n * (S + (copy ? 8 : 0));
             }
+            if (!grow) kept += n_cur;
         }
         CK(cudaMemcpy(counts, d0, 16, cudaMemcpyDeviceToHost));
-        kept = counts[0];
+        if (grow) kept = counts[0];
         if (kept > fcap_total) {
             snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (recover): rank %d of %d owns %llu of the checkpoint's frontier states, its frontier holds %llu",
                      me, W, (unsigned long long)kept, (unsigned long long)fcap_total);
@@ -529,57 +465,68 @@ int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, 
         }
         if (counts[1]) {
             snprintf(e->last_error, sizeof e->last_error,
-                     "recover: the checkpoint's frontier and seen-set disagree: %llu frontier states rank %d owns are not in its seen-set at depth %d", counts[1], me, h[0].level);
+                     "recover: the checkpoint's frontier and seen-set disagree: %llu frontier states rank %d took are not in its seen-set at depth %d", counts[1], me,
+                     h[0].level);
             return VSR_RC_ERROR;
         }
         if (tr && cur_base + kept > e->trace.capacity()) {
             snprintf(e->last_error, sizeof e->last_error,
-                     "capacity exceeded (recover): rank %d needs %llu trace records (%llu of the checkpoint's %llu, then %llu frontier copies), it holds %llu", me,
-                     (unsigned long long)(cur_base + kept), (unsigned long long)cur_base, (unsigned long long)T, (unsigned long long)kept, (unsigned long long)e->trace.capacity());
+                     "capacity exceeded (recover): rank %d needs %llu trace records (%llu of the checkpoint's %llu, then %llu frontier states), it holds %llu", me,
+                     (unsigned long long)(cur_base + kept), (unsigned long long)cur_base, (unsigned long long)T, (unsigned long long)kept,
+                     (unsigned long long)e->trace.capacity());
             return VSR_RC_TOO_LARGE;
         }
     }
-    /* 5. this rank's slice [lo, hi) of the old records, from whichever files hold it, renumbered on the device */
-    if (e->trace_cap && h[0].keep_trace) {
+    /* 5. this rank's old records [lo, hi) of each source file, renumbered on the device: each chunk lies on one side of
+       the file's cut, where the new ids are consecutive */
+    if (tr) {
         const uint64_t per = std::max<uint64_t>(1, std::min(IO_CHUNK, scratch_bytes) / 8);
         host.resize(per * 8);
-        for (int r = 0; r < Wold; r++) {
-            const uint64_t a = std::max<uint64_t>(lo, m.off[r]), b = std::min<uint64_t>(hi, m.off[r] + h[r].next_base);
-            if (a >= b) continue;
-            if ((rc = seek(e, in[r], trace_at(h[r]) + (a - m.off[r]) * 8, files[r].c_str()))) return rc;
-            for (uint64_t o = a; o < b; o += per) {
-                const uint64_t k = std::min(per, b - o);
+        for (int r = src; r < src + nsrc; r++) {
+            const uint64_t a = grow ? lo : 0, b = grow ? hi : h[r].next_base;
+            if (a < b && (rc = seek(e, in[r], trace_at(h[r]) + a * 8, files[r].c_str()))) return rc;
+            for (uint64_t o = a, n; o < b; o += n) {
+                n = std::min(per, (o < m.cut[r] ? std::min<uint64_t>(b, m.cut[r]) : b) - o);
                 double t = now_s();
-                if (fread(host.data(), 8, k, in[r].f) != k) return io_error(e, "truncated", files[r].c_str());
+                if (fread(host.data(), 8, n, in[r].f) != n) return io_error(e, "truncated", files[r].c_str());
                 t_read += now_s() - t;
                 t = now_s();
-                CK(cudaMemcpyAsync(scratch, host.data(), k * 8, cudaMemcpyHostToDevice, e->stream));
-                ckpt_remap_trace_kernel<<<e->sms * 4, 256, 0, e->stream>>>((const uint64_t*)scratch, k, e->trace.view().from(o - lo, 2), m);
+                const uint64_t row = remap_gid(m, make_gid(r, o)) & ((1ull << 40) - 1ull);
+                CK(cudaMemcpyAsync(scratch, host.data(), n * 8, cudaMemcpyHostToDevice, e->stream));
+                ckpt_remap_trace_kernel<<<e->sms * 4, 256, 0, e->stream>>>((const uint64_t*)scratch, n, e->trace.view().from(row, 2), m);
                 CK(cudaGetLastError());
                 CK(cudaStreamSynchronize(e->stream));
                 t_trace += now_s() - t;
-                bytes_read += k * 8;
-                e->st.bytes_h2d += k * 8;
+                bytes_read += n * 8;
             }
         }
     }
-    /* the BFS position: the frontier of depth `level`, this rank's ids continue after its slice */
-    e->st.distinct = owned;
+    /* the BFS position: the frontier of depth `level`, this rank's ids continue after it */
+    if (W == Wold) { /* the same world: this rank's counters continue; capacities are this engine's */
+        const VsrStats fresh = e->st;
+        e->st = mine;
+        e->st.table_capacity = fresh.table_capacity; e->st.frontier_capacity = fresh.frontier_capacity;
+        e->st.bytes_table = fresh.bytes_table; e->st.bytes_frontier = fresh.bytes_frontier;
+        e->records_sent = h[me].records_sent; e->records_received = h[me].records_received;
+    } else {
+        e->st.distinct = owned;
+        e->st.kernel_launches = launches;
+    }
+    e->st.bytes_h2d += bytes_read;
     e->n_cur = kept;
     e->cur_base = cur_base;
     e->next_base = cur_base + kept;
     e->cur = 0;
     e->level = h[0].level;
     e->level_open = false;
-    if (e->opts.collect_levels) e->collected.resize(h[0].level);
-    e->records_sent = e->records_received = 0;
+    if (e->opts.collect_levels) e->collected.resize(h[0].level); /* depths up to the checkpoint's were collected by another run: empty */
     if (tot.violation_level) tot.violation_id = remap_gid(m, tot.violation_id);
     if (totals_out) *totals_out = tot;
     if (e->opts.verbose)
         fprintf(stderr,
                 "recover: rank %d of %d took its share of %d checkpoint files (%llu bytes read) in %.3f s: %.3f s reading, %.3f s seen-set insert, %.3f s frontier, %.3f s trace; "
                 "%llu seen-set entries, %llu frontier states\n",
-                me, W, Wold, (unsigned long long)bytes_read, now_s() - t_start, t_read, t_insert, t_frontier, t_trace, (unsigned long long)owned,
+                me, W, nsrc, (unsigned long long)bytes_read, now_s() - t_start, t_read, t_insert, t_frontier, t_trace, (unsigned long long)owned,
                 (unsigned long long)kept);
     return 0;
 }

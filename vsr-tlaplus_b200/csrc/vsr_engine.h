@@ -10,7 +10,6 @@
 #include <string.h>
 
 #include <chrono>
-#include <string>
 #include <vector>
 
 #include "vsr_gpu_thunks.cuh"
@@ -97,11 +96,6 @@ int live_create(VsrEngine* e, char* err, size_t errcap);
 void live_destroy(VsrEngine* e);
 int live_reset(VsrEngine* e);
 int live_collect(VsrEngine* e);
-/* vsr_ckpt.cu: recovery on another number of ranks.  ckpt_old_files: the files of the checkpoint at `base` when they were
-   written by another number of ranks than e's world (empty: this world's own files, vsr_engine_recover reads them; 151 when
-   a one-rank and a several-rank checkpoint both lie there).  ckpt_recover_resharded: this rank's share of all of them. */
-int ckpt_old_files(VsrEngine* e, const char* base, std::vector<std::string>& files);
-int ckpt_recover_resharded(VsrEngine* e, const std::vector<std::string>& files, VsrStats* totals_out);
 /* vsr_shard.cu: the candidate chain from Init to global state id `gid` (every rank of a group calls it together) */
 int walk_trace(VsrEngine* e, uint64_t gid, std::vector<uint32_t>& cands);
 

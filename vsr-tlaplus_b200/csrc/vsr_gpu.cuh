@@ -1081,21 +1081,27 @@ template <class L> __global__ void audit_frontier_kernel(const ExpandParams P, c
     audit_add(&out->words_xor, wx, true);
 }
 
-/* ------------------------------------------------------------------ re-sharding a checkpoint (vsr_ckpt.cu)
-   A checkpoint written by W_old ranks, continued by W_new ranks.  Every old trace record gets a place in one global order,
-   F(r, l) = off[r] + l (off = prefix sum of the old files' record counts), and the new world cuts that order into slices of
-   `slice` records: F lands on rank F / slice at local id F % slice.  Every stored global id (trace parents, the totals'
-   violation id) is renumbered with this one function, so the parent walk reads the new ids as it read the old ones. */
+/* ------------------------------------------------------------------ recovering a checkpoint (vsr_ckpt.cu)
+   A checkpoint written by W_old ranks, continued by W_new ranks (both powers of two).  Old record l of old rank q gets its
+   new global id from five per-old-rank numbers:
+     l < cut[q]:  rank to[q] + l / slice[q], local id hist[q] + l % slice[q]
+     else:        rank to[q], local id front[q] + l - cut[q]
+   Shrinking or the same world (W_old = k W_new): new rank q / k holds its group's histories (slice and cut: hist = ids of
+   the group's earlier files, cut = cur_base), then its group's frontiers (front); with k = 1 this is the identity.  Growing
+   (W_new = s W_old): file q's records are cut into s slices of ceil(next_base / s) (cut = infinity).  Every stored global
+   id (trace parents, the totals' violation id) is renumbered with this one function, so the parent walk reads the new ids
+   as it read the old ones. */
+constexpr unsigned long long REMAP_ALL = ~0ull; /* slice or cut: infinity */
 struct GidRemap {
-    unsigned long long off[MAX_WORLD]; /* off[r] = records of the old ranks before r */
-    unsigned long long slice;          /* records per new rank (ceil(total / W_new); >= 1) */
+    unsigned long long slice[MAX_WORLD], hist[MAX_WORLD], cut[MAX_WORLD], front[MAX_WORLD];
+    int to[MAX_WORLD];
     int old_world, _pad;
 };
 __host__ __device__ __forceinline__ uint64_t remap_gid(const GidRemap& m, uint64_t gid) {
     if (gid == ROOT_GID) return ROOT_GID;
-    const int r = (int)(gid >> 40);
-    const unsigned long long F = m.off[r < m.old_world ? r : 0] + (gid & ((1ull << 40) - 1ull));
-    return make_gid((int)(F / m.slice), F % m.slice);
+    const int r = (int)(gid >> 40), q = r < m.old_world ? r : 0;
+    const unsigned long long l = gid & ((1ull << 40) - 1ull);
+    return l < m.cut[q] ? make_gid(m.to[q] + (int)(l / m.slice[q]), m.hist[q] + l % m.slice[q]) : make_gid(m.to[q], m.front[q] + l - m.cut[q]);
 }
 __host__ __device__ __forceinline__ uint64_t remap_trec(const GidRemap& m, uint64_t t) {
     return make_trec(remap_gid(m, (t >> 12) & GID_MASK), (uint32_t)(t & 0xFFFu));
@@ -1108,20 +1114,23 @@ struct ReshardParams {
     unsigned long long n;
     SpillRows out;                     /* frontier buffer 0 */
     unsigned long long out_cap;
+    unsigned long long out_first;      /* place: state i goes to row out_first + i */
     SpillRows trace;                   /* record of kept state j goes to row trace_base + j */
-    unsigned long long trace_base, trace_cap; /* trace_cap 0: no trace */
-    const uint64_t* table;             /* this rank's seen-set, already filled from every old file */
+    unsigned long long trace_base, trace_cap; /* trace_cap 0: no trace (or place: the records are already in place) */
+    const uint64_t* table;             /* this rank's seen-set, already filled from its source files */
     unsigned long long table_cap;
     const uint64_t* fp_tab;
     RunCfg run;
-    int rank, owner_shift, level, _pad;
+    int rank, owner_shift, level, place; /* place: shrinking or the same world, where every state of the chunk is this rank's */
     GidRemap remap;
-    unsigned long long* kept;          /* states this rank owns, over all chunks (their positions in buffer 0) */
-    unsigned long long* missing;       /* owned states not in the seen-set with the checkpoint's level */
+    unsigned long long* kept;          /* !place: states this rank owns, over all chunks (their positions in buffer 0) */
+    unsigned long long* missing;       /* states kept that are not in the seen-set with the checkpoint's level (place: or not owned) */
 };
-/* Keep the states this rank owns — the expand kernel's fingerprint and owner rule — and append them to frontier buffer 0
-   (one atomic per warp), each with its trace record renumbered.  Every kept state must already be in the seen-set at the
-   checkpoint's level: a miss means the files disagree, and the host refuses the recovery. */
+/* Keep the states this rank owns — the expand kernel's fingerprint and owner rule.  place: every state of the chunk is this
+   rank's and goes to its row, with no atomics and no record copy (its record was loaded with the trace).  Else the owned
+   states are appended to frontier buffer 0 (one atomic per warp), each with its trace record renumbered.  Every kept state
+   must already be in the seen-set at the checkpoint's level: a miss (or, placed, a state of another rank) means the files
+   disagree, and the host refuses the recovery. */
 template <class L> __global__ void reshard_frontier_kernel(const ReshardParams P) {
     const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
     const unsigned long long rounds = (P.n + stride - 1) / stride;
@@ -1136,17 +1145,23 @@ template <class L> __global__ void reshard_frontier_kernel(const ReshardParams P
             uint64_t fp = fp64_view8<L>(P.fp_tab, w, P.run.use_view != 0);
             if (fp == 0) fp = 1;
             mine = owner_of(fp, P.owner_shift) == P.rank;
-            if (mine && (int)(table_lookup(P.table, P.table_cap, fp, check_hash<L>(w, P.run.use_view != 0)) >> 56) != P.level) miss++;
+            if (mine ? (int)(table_lookup(P.table, P.table_cap, fp, check_hash<L>(w, P.run.use_view != 0)) >> 56) != P.level : P.place != 0) miss++;
         }
-        const unsigned m = __ballot_sync(0xffffffffu, mine);
-        if (!m) continue;
-        unsigned long long base = 0;
-        const int leader = __ffs(m) - 1;
-        if (lane == leader) base = atomicAdd(P.kept, (unsigned long long)__popc(m));
-        base = __shfl_sync(0xffffffffu, base, leader);
-        if (!mine) continue;
-        const unsigned long long pos = base + __popc(m & ((1u << lane) - 1u));
-        if (pos >= P.out_cap) continue; /* counted: the host reports the owned frontier's size */
+        unsigned long long pos;
+        if (P.place) { /* the same for the whole grid: no ballot below */
+            if (i >= P.n) continue;
+            pos = P.out_first + i;
+        } else {
+            const unsigned m = __ballot_sync(0xffffffffu, mine);
+            if (!m) continue;
+            unsigned long long base = 0;
+            const int leader = __ffs(m) - 1;
+            if (lane == leader) base = atomicAdd(P.kept, (unsigned long long)__popc(m));
+            base = __shfl_sync(0xffffffffu, base, leader);
+            if (!mine) continue;
+            pos = base + __popc(m & ((1u << lane) - 1u));
+        }
+        if (pos >= P.out_cap) continue; /* counted: the host reports the frontier's size */
         uint32_t* dst = P.out.row<L::NW>(pos);
         for (int j = 0; j < L::NW; j++) dst[j] = w[j];
         if (P.trace_base + pos < P.trace_cap) *(uint64_t*)P.trace.row<2>(P.trace_base + pos) = remap_trec(P.remap, P.in_trace[i]);

@@ -269,35 +269,29 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     bool complete = false, bounded = false;
     uint64_t bad_gid = ~0ull;
     double kernel_ms = 0, insert_ms = 0;
-    /* checkpoints: with several ranks every rank writes / reads <path>.rank<r> at the same level boundary (rank 0's clock
-       decides when); one rank uses <path> itself */
-    auto rank_file = [&](const char* path) { return W > 1 ? std::string(path) + ".rank" + std::to_string(me) : std::string(path); };
-    const std::string ckpt_path = opts->checkpoint_path ? rank_file(opts->checkpoint_path) : std::string();
+    /* checkpoints: with several ranks every rank writes <path>.rank<r> at the same level boundary (rank 0's clock decides
+       when); one rank writes <path> itself */
+    const std::string ckpt_path = !opts->checkpoint_path ? std::string()
+                                : W > 1 ? std::string(opts->checkpoint_path) + ".rank" + std::to_string(me) : std::string(opts->checkpoint_path);
     const std::string slowest = W > 1 ? " (slowest of " + std::to_string(W) + " GPUs)" : "";
     double last_ckpt = now_s();
     bool resumed = false;
     int rc;
     if (opts->recover_path) {
-        /* a checkpoint of this world: each rank reads its own file.  Of another world: each rank reads every old file and
-           keeps its share (vsr_ckpt.cu).  Every rank takes the same choice from the same files */
-        std::vector<std::string> old;
-        rc = ckpt_old_files(e, opts->recover_path, old);
-        if (!rc && old.empty()) rc = vsr_engine_recover(e, rank_file(opts->recover_path).c_str(), &tot);
-        else if (!rc) {
-            rc = ckpt_recover_resharded(e, old, &tot);
-            if (W > 1) { /* a share that does not fit fails on its rank only: all report the first failure, with its message */
-                RecoverMsg rm, rms[MAX_WORLD];
-                memset(&rm, 0, sizeof rm);
-                rm.rc = rc;
-                if (rc) memcpy(rm.msg, e->last_error, sizeof rm.msg - 1);
-                if (vsr_group_allgather(g, &rm, sizeof rm, rms)) return set_error(e, "%s", g->last_error);
-                for (int r = 0; r < W; r++)
-                    if (rms[r].rc) {
-                        if (!rc) snprintf(e->last_error, sizeof e->last_error, "%s", rms[r].msg);
-                        rc = rms[r].rc;
-                        break;
-                    }
-            }
+        /* each rank loads its share of a checkpoint of any world (vsr_ckpt.cu) */
+        rc = vsr_engine_recover(e, opts->recover_path, &tot);
+        if (W > 1) { /* a share that does not fit fails on its rank only: all report the first failure, with its message */
+            RecoverMsg rm, rms[MAX_WORLD];
+            memset(&rm, 0, sizeof rm);
+            rm.rc = rc;
+            if (rc) memcpy(rm.msg, e->last_error, sizeof rm.msg - 1);
+            if (vsr_group_allgather(g, &rm, sizeof rm, rms)) return set_error(e, "%s", g->last_error);
+            for (int r = 0; r < W; r++)
+                if (rms[r].rc) {
+                    if (!rc) snprintf(e->last_error, sizeof e->last_error, "%s", rms[r].msg);
+                    rc = rms[r].rc;
+                    break;
+                }
         }
         if (!rc) {
             resumed = true;

@@ -175,8 +175,8 @@ class GpuEngine:
             want_trace: bool = True, part_states: int = 0, verbose: bool = False, checkpoint_path: Optional[str] = None,
             recover_path: Optional[str] = None, checkpoint_seconds: float = 0.0) -> ShardedResult:
         """checkpoint_path / recover_path: written / read at level boundaries (TLC -checkpoint / -recover); with several ranks
-        every rank uses ``<path>.rank<r>``.  recover_path may have been written by any number of ranks: every rank then reads
-        all the old files and keeps its own share.  Not with exchange="staged": that engine cannot run this loop."""
+        every rank uses ``<path>.rank<r>``.  recover_path (the base path) may have been written by any number of ranks: every
+        rank reads the files that hold its own share.  Not with exchange="staged": that engine cannot run this loop."""
         o = self._opts
         o.max_depth, o.max_seconds, o.max_states = max_depth, max_seconds, max_states
         o.stop_on_violation, o.verbose = int(stop_on_violation), int(verbose)
