@@ -79,7 +79,10 @@ int vsr_load_cfg_text(const char* cfg_text, const char* tla_path, VsrModel** out
  * bits only this entry point knows: 512 = check PROPERTY ViewChangeCompletes (as a cfg with SPECIFICATION Spec does); test
  * hooks of the liveness pass, which leave the BFS as it is: 1024 = the pass checks []<>Q with Q = "some replica's
  * rep_commit_number >= 1" instead (reachable not-Q states without successors exist), 2048 = in the pass every state
- * without successors gets one extra successor, Init (with 1024: cycles through Init) */
+ * without successors gets one extra successor, Init (with 1024: cycles through Init); 4096 = the INVARIANT list names
+ * AcknowledgedWritesExistOnMajority before AcknowledgedWriteNotLost (otherwise the list is in bit order), which decides
+ * the name vsr_reported_invariant gives a state that violates both.  Test hook 256: the invariant "no replica has
+ * committed every value", reported in the masks as 256 (vsr_reported_invariant does not name it) */
 int vsr_model_create(int replica_count, int client_count, int value_count, int start_view_on_timer_limit,
                      int restart_empty_limit, int symmetry, int view, int invariant, VsrModel** out, char* err,
                      size_t errcap);
@@ -105,7 +108,11 @@ uint32_t vsr_aux_key(const VsrModel* m, const void* state);
 /* rank (GPU) that owns a fingerprint when the state space is sharded over `world` = 1, 2, 4 or 8 ranks: the high bits of
  * fingerprint x an odd constant (FP64 is GF(2)-linear: its own high bits would route a rank's successors to a few peers only) */
 int vsr_owner_rank(uint64_t fingerprint, int world);
-int vsr_invariant(const VsrModel* m, const void* state);                 /* 0 = all hold, else mask bit of the violated one; VSR.tla:926-952 */
+/* invariants, VSR.tla:926-952: the mask of the configured INVARIANT bits the state violates (0 = all hold), all of them */
+int vsr_invariant(const VsrModel* m, const void* state);
+/* the invariant TLC names for the state ("Error: Invariant X is violated."): the first of the config's INVARIANT list, in
+ * its order, that the state violates; NULL if it violates none */
+const char* vsr_reported_invariant(const VsrModel* m, const void* state);
 /* 1 if the state predicate the liveness pass checks holds in `state`: AllReplicasMoveToSameView (VSR.tla:958-962), or the
  * test hook's Q (vsr_model_create bit 1024); 0 if not */
 int vsr_property(const VsrModel* m, const void* state);
@@ -186,7 +193,7 @@ typedef struct VsrStats {
     int32_t violation_level;              /* depth of the violating state */
     int32_t trace_len;
     int32_t error_code;                   /* first E_* raised on the device (0 = none) */
-    int32_t violation_mask;               /* INVARIANT bits violated by the reported state (0 = none reported) */
+    int32_t violation_mask;               /* every INVARIANT bit the reported state violates (vsr_invariant; 0 = none reported) */
     uint64_t violation_id;
     uint64_t table_capacity, frontier_capacity;
     uint64_t bytes_table, bytes_frontier;
@@ -205,7 +212,8 @@ typedef struct VsrEngine VsrEngine;
  * back edge), teardown.
  * Fails loudly (153) when no CUDA device is usable — there is no CPU fallback.  If trace_out != NULL and a
  * violation/deadlock is found, writes the counterexample (packed states, trace_cap capacity) with its action ids;
- * stats.trace_len is its length, stats.violation_mask the invariants its last state violates. */
+ * stats.trace_len is its length, stats.violation_mask the invariants its last state violates (all of them: the one TLC
+ * names is vsr_reported_invariant of that state). */
 int vsr_bfs(const VsrModel* m, const VsrRunOpts* opts, VsrStats* stats, void* trace_out, uint8_t* trace_actions,
             size_t trace_cap);
 
@@ -239,7 +247,7 @@ typedef struct VsrLevelInfo {
     uint64_t violation_id, deadlock_id;
     double ms;        /* kernel time of the level on this rank (expand + insert), CUDA events on the launch stream */
     double ms_insert; /* of which launches that only inserted records received from peers */
-    int32_t violation_mask, _pad; /* INVARIANT bits (VsrModelInfo.invariant) violated by some new state of the level */
+    int32_t violation_mask, _pad; /* OR over the level's new states of the INVARIANT bits each violates (vsr_invariant) */
 } VsrLevelInfo;
 int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out);
 uint64_t vsr_engine_frontier_size(const VsrEngine* e);

@@ -172,7 +172,7 @@ class VsrLevelAudit(C.Structure):
 # every symbol include/vsr_b200.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = [
     "vsr_load", "vsr_load_cfg_text", "vsr_model_create", "vsr_model_free", "vsr_model_info", "vsr_init", "vsr_successors", "vsr_enabled_candidates",
-    "vsr_canon", "vsr_fingerprint", "vsr_fingerprint_bytewise", "vsr_aux_key", "vsr_owner_rank", "vsr_invariant", "vsr_property", "vsr_unpack", "vsr_pack", "vsr_state_to_tla",
+    "vsr_canon", "vsr_fingerprint", "vsr_fingerprint_bytewise", "vsr_aux_key", "vsr_owner_rank", "vsr_invariant", "vsr_reported_invariant", "vsr_property", "vsr_unpack", "vsr_pack", "vsr_state_to_tla",
     "vsr_flat_to_tla", "vsr_action_name", "vsr_action_location", "vsr_bfs", "vsr_engine_create", "vsr_engine_destroy",
     "vsr_engine_record_bytes", "vsr_engine_seed_init", "vsr_engine_expand", "vsr_engine_expand_part", "vsr_engine_step",
     "vsr_engine_insert_records", "vsr_engine_finish_level", "vsr_engine_frontier_size", "vsr_engine_read_frontier",
@@ -215,6 +215,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
     lib.vsr_owner_rank.argtypes = [u64, C.c_int]
     lib.vsr_aux_key.restype = C.c_uint32
     lib.vsr_invariant.argtypes = [vp, vp]
+    lib.vsr_reported_invariant.argtypes = [vp, vp]
+    lib.vsr_reported_invariant.restype = cp
     lib.vsr_property.argtypes = [vp, vp]
     lib.vsr_engine_liveness.argtypes = [vp, C.POINTER(VsrLiveStats), C.POINTER(C.c_uint32), C.c_size_t]
     lib.vsr_unpack.argtypes = [vp, vp, C.POINTER(VsrFlatState)]
@@ -353,7 +355,8 @@ class CheckResult:
     bytes_h2d: int = 0
     bytes_d2h: int = 0
     seconds_setup: float = 0.0
-    violated_invariants: List[str] = field(default_factory=list)  # names of the INVARIANTs the reported state violates
+    # rc 12: the one invariant TLC names for the reported state, the first of the INVARIANT list it violates ([] = none named)
+    violated_invariants: List[str] = field(default_factory=list)
     records_sent: int = 0        # several GPUs: records this rank pushed to peers / drained from its inbox
     records_received: int = 0
     seconds_insert: float = 0.0
@@ -419,6 +422,10 @@ class ModelChecker:
         mask = 0
         for n in invariants:
             mask |= INVARIANT_BITS[n]
+        names = list(invariants)
+        if {"AcknowledgedWriteNotLost", "AcknowledgedWritesExistOnMajority"} <= set(names) and \
+                names.index("AcknowledgedWritesExistOnMajority") < names.index("AcknowledgedWriteNotLost"):
+            mask |= 4096  # the list's order decides which of the two TLC names for a state violating both
         mask |= (512 if property else 0) | (1024 if live_test_hooks & 1 else 0) | (2048 if live_test_hooks & 2 else 0)
         rc = lib.vsr_model_create(replica_count, client_count, value_count, start_view_on_timer_limit, restart_empty_limit,
                                   int(symmetry), int(view), mask, C.byref(h), err, len(err))
@@ -474,7 +481,13 @@ class ModelChecker:
         return int(self._lib.vsr_aux_key(self._h, (C.c_uint8 * self.state_bytes).from_buffer_copy(state)))
 
     def invariant(self, state: bytes) -> int:
+        """mask of the configured invariants the state violates (INVARIANT_BITS; 256 = the test hook), 0 if all hold"""
         return int(self._lib.vsr_invariant(self._h, (C.c_uint8 * self.state_bytes).from_buffer_copy(state)))
+
+    def reported_invariant(self, state: bytes) -> Optional[str]:
+        """the invariant TLC names for the state: the first of the INVARIANT list, in its order, that it violates"""
+        name = self._lib.vsr_reported_invariant(self._h, (C.c_uint8 * self.state_bytes).from_buffer_copy(state))
+        return name.decode() if name else None
 
     def property_holds(self, state: bytes) -> bool:
         """the state predicate the liveness pass checks (AllReplicasMoveToSameView, or the test hook's Q)"""
@@ -561,9 +574,9 @@ class ModelChecker:
         o.checkpoint_seconds = checkpoint_seconds
         return o
 
-    @staticmethod
-    def result_from_stats(st: VsrStats, rc: int, trace=None, levels=None) -> CheckResult:
+    def result_from_stats(self, st: VsrStats, rc: int, trace=None, levels=None) -> CheckResult:
         n = int(st.num_levels)
+        name = self.reported_invariant(trace[-1][1]) if rc == 12 and trace else None
         return CheckResult(
             rc=rc, generated=int(st.generated), distinct=int(st.distinct), queue=int(st.queue), depth=int(st.depth),
             complete=bool(st.complete), level_sizes=[int(st.level_sizes[i]) for i in range(n)],
@@ -573,7 +586,7 @@ class ModelChecker:
             seconds_kernels=float(st.seconds_kernels), violation_level=int(st.violation_level), error_code=int(st.error_code),
             table_capacity=int(st.table_capacity), frontier_capacity=int(st.frontier_capacity), bytes_h2d=int(st.bytes_h2d),
             bytes_d2h=int(st.bytes_d2h), seconds_setup=float(st.seconds_setup),
-            violated_invariants=[n for n, b in INVARIANT_BITS.items() if int(st.violation_mask) & b],
+            violated_invariants=[name] if name else [],
             records_sent=int(st.records_sent), records_received=int(st.records_received), seconds_insert=float(st.seconds_insert),
             trace=trace or [], levels=levels or [])
 
@@ -685,8 +698,6 @@ class ModelChecker:
                 lib.vsr_engine_collected(e, lv, buf, k)
                 levels.append(bytes(buf))
             trace = self._trace_from_cands(cands, n.value) if st.trace_len else []
-            if rc == 12 and trace:
-                st.violation_mask = self.invariant(trace[-1][1])
             live = {}
             if rc == 0 and st.complete and self.info.property:
                 ls = VsrLiveStats()

@@ -526,14 +526,16 @@ template <class L> struct Ops {
         }
     }
 
-    /* invariants, VSR.tla:926-952; returns 0 if all selected hold, else the mask bit of the violated one */
+    /* invariants, VSR.tla:926-952; returns the mask of the selected ones the state violates (0 = all hold).  Every value is
+       visited: a state can violate both, and which one TLC names depends on the INVARIANT order (vsr_reported_invariant) */
     template <class W> static VSR_HD int invariant(const RunCfg& run, const W& w) {
+        int bad = 0;
         if (run.invariant & 256) { /* test hook, not a spec invariant (only reachable through vsr_model_create): "no replica has
                                       committed every value" — violated often, so tests can exercise the violation paths */
             for (int r = 0; r < R; r++)
-                if ((int)VGET(L, COMMIT, w, r) == V) return 256;
+                if ((int)VGET(L, COMMIT, w, r) == V) bad = 256;
         }
-        if (!(run.invariant & 3)) return 0; /* NoLogDivergence is vacuous (r1/r1, :931), TestInv is TRUE */
+        if (!(run.invariant & 3)) return bad; /* NoLogDivergence is vacuous (r1/r1, :931), TestInv is TRUE */
         for (int x = 0; x < V; x++) {
             if (VGET(L, ACKED, w, x) != ACK_TRUE) continue;
             int holders = 0;
@@ -542,10 +544,10 @@ template <class L> struct Ops {
                 for (int i = 0; i < V; i++) has |= (int)VGET(L, LOG, w, r * V + i) == x + 1; /* ReplicaHasOp :933-935 */
                 holders += has;
             }
-            if ((run.invariant & 1) && holders == 0) return 1;         /* AcknowledgedWriteNotLost :945-950 */
-            if ((run.invariant & 2) && holders < R / 2 + 1) return 2;  /* AcknowledgedWritesExistOnMajority :937-943 */
+            if ((run.invariant & 1) && holders == 0) bad |= 1;         /* AcknowledgedWriteNotLost :945-950 */
+            if ((run.invariant & 2) && holders < R / 2 + 1) bad |= 2;  /* AcknowledgedWritesExistOnMajority :937-943 */
         }
-        return 0;
+        return bad;
     }
 
     /* AllReplicasMoveToSameView, VSR.tla:958-962: every replica is Normal and all have the same view number.  The state

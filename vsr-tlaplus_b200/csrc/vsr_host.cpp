@@ -497,12 +497,14 @@ static int parse_cfg(const std::string& text, VsrModel* m, std::string& why) {
     if (!view.empty() && view != "view") { why = "VIEW `" + view + "` unknown; VSR.tla defines `view` (:149)"; return VSR_RC_CONFIG_ERROR; }
     if (!symm.empty() && symm != "symmValues") { why = "SYMMETRY `" + symm + "` unknown; VSR.tla defines `symmValues` (:151)"; return VSR_RC_CONFIG_ERROR; }
     int mask = 0;
+    m->inv_order.clear();
     for (const std::string& s : invs) {
-        if (s == "AcknowledgedWriteNotLost") mask |= 1;
-        else if (s == "AcknowledgedWritesExistOnMajority") mask |= 2;
-        else if (s == "NoLogDivergence") mask |= 4;
-        else if (s == "TestInv") mask |= 8;
-        else { why = "INVARIANT `" + s + "` is not defined in VSR.tla (:926-952)"; return VSR_RC_CONFIG_ERROR; }
+        int bit = 0;
+        for (int b = 0; b < 4; b++)
+            if (s == INVARIANT_NAMES[b]) bit = 1 << b;
+        if (!bit) { why = "INVARIANT `" + s + "` is not defined in VSR.tla (:926-952)"; return VSR_RC_CONFIG_ERROR; }
+        if (!(mask & bit)) m->inv_order.push_back(bit);
+        mask |= bit;
     }
     VsrModelInfo& I = m->info;
     I.replica_count = ints["ReplicaCount"];
@@ -852,8 +854,11 @@ int vsr_model_create(int R, int C, int V, int L, int restart, int symmetry, int 
     VsrModelInfo& I = m->info;
     I.replica_count = R; I.client_count = C; I.value_count = V; I.start_view_on_timer_limit = L; I.restart_empty_limit = restart;
     I.symmetry = symmetry ? 1 : 0; I.view = view ? 1 : 0;
-    I.invariant = invariant & ~(MODEL_PROPERTY_BIT | MODEL_HOOK_Q_BIT | MODEL_HOOK_INIT_EDGE_BIT);
+    I.invariant = invariant & ~(MODEL_PROPERTY_BIT | MODEL_HOOK_Q_BIT | MODEL_HOOK_INIT_EDGE_BIT | MODEL_MAJORITY_FIRST_BIT);
     I.property = (invariant & MODEL_PROPERTY_BIT) ? 1 : 0;
+    static const int order[2][4] = {{1, 2, 4, 8}, {2, 1, 4, 8}};
+    for (int b : order[(invariant & MODEL_MAJORITY_FIRST_BIT) ? 1 : 0])
+        if (I.invariant & b) m->inv_order.push_back(b);
     m->live_hooks = ((invariant & MODEL_HOOK_Q_BIT) ? LIVE_HOOK_Q : 0) | ((invariant & MODEL_HOOK_INIT_EDGE_BIT) ? LIVE_HOOK_INIT_EDGE : 0);
     if (V < 1 || V > VSR_MAX_V) { set_err(err, errcap, "|Values| out of range"); delete m; return VSR_RC_CONFIG_ERROR; }
     for (int v = 0; v < V; v++) snprintf(I.value_names[v], sizeof I.value_names[v], "v%d", v + 1);
@@ -920,6 +925,12 @@ int vsr_owner_rank(uint64_t fingerprint, int world) {
     return vsr::owner_of(fingerprint ? fingerprint : 1, 64 - lg);
 }
 int vsr_invariant(const VsrModel* m, const void* s) { return m->ops->invariant(&m->run, (const uint32_t*)s); }
+const char* vsr_reported_invariant(const VsrModel* m, const void* s) {
+    const int bad = vsr_invariant(m, s);
+    for (int b : m->inv_order)
+        if (bad & b) return INVARIANT_NAMES[__builtin_ctz((unsigned)b)];
+    return nullptr;
+}
 int vsr_property(const VsrModel* m, const void* s) { return m->ops->property(&m->run, (const uint32_t*)s, m->live_hooks); }
 int vsr_unpack(const VsrModel* m, const void* s, VsrFlatState* out) { return m->ops->unpack((const uint32_t*)s, out); }
 int vsr_pack(const VsrModel* m, const VsrFlatState* in, void* s) { return m->ops->pack(in, (uint32_t*)s, m->run.symmetry); }

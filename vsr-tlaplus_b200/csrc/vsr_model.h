@@ -6,6 +6,7 @@
 #define VSR_MODEL_H
 
 #include <string>
+#include <vector>
 
 #include "../../include/vsr_b200.h"
 #include "vsr_actions.h"
@@ -24,8 +25,12 @@ namespace vsr {
 
 struct GpuOps; /* vsr_gpu.cu */
 
-/* vsr_model_create's `invariant` bits above the INVARIANT mask (include/vsr_b200.h) */
-enum { MODEL_PROPERTY_BIT = 512, MODEL_HOOK_Q_BIT = 1024, MODEL_HOOK_INIT_EDGE_BIT = 2048 };
+/* vsr_model_create's `invariant` bits above the INVARIANT mask (include/vsr_b200.h).  MODEL_MAJORITY_FIRST_BIT is the whole
+   INVARIANT order this entry point can express: NoLogDivergence (4) and TestInv (8) never fail (VSR.tla:926-931, :952), so
+   only the order of bits 1 and 2 can change the name reported; a third invariant that can fail needs a full order here */
+enum { MODEL_PROPERTY_BIT = 512, MODEL_HOOK_Q_BIT = 1024, MODEL_HOOK_INIT_EDGE_BIT = 2048, MODEL_MAJORITY_FIRST_BIT = 4096 };
+/* names of the INVARIANT mask bits 1, 2, 4, 8 */
+static const char* const INVARIANT_NAMES[4] = {"AcknowledgedWriteNotLost", "AcknowledgedWritesExistOnMajority", "NoLogDivergence", "TestInv"};
 enum { LIVE_HOOK_Q = 1, LIVE_HOOK_INIT_EDGE = 2 };
 
 struct ModelOps {
@@ -62,6 +67,7 @@ struct VsrModel {
     const vsr::GpuOps* gpu;
     int check_deadlock_cfg; /* CHECK_DEADLOCK in the cfg: -1 unset */
     int live_hooks = 0;     /* test hooks of the liveness pass (vsr_model_create): LIVE_HOOK_* */
+    std::vector<int> inv_order; /* INVARIANT mask bits in the config's order: TLC reports the first one a state violates */
     std::string action_location[VSR_NUM_ACTIONS];
 };
 

@@ -246,6 +246,16 @@ class GpuEngine:
     def frontier_size(self) -> int:
         return int(self.lib.vsr_engine_frontier_size(self._e))
 
+    def read_frontier(self, first: int = 0, n: Optional[int] = None) -> bytes:
+        """packed states [first, first + n) of the current frontier (n = None: to its end); after finish() row i is the state
+        with local id (states of the earlier levels) + i"""
+        if n is None:
+            n = max(self.frontier_size() - first, 0)
+        buf = (C.c_uint8 * max(n * self.mc.state_bytes, 1))()
+        if n:
+            self._ck(self.lib.vsr_engine_read_frontier(self._e, first, n, buf))
+        return bytes(buf)[: n * self.mc.state_bytes]
+
     def stats(self) -> "ck.VsrStats":
         st = ck.VsrStats()
         self.lib.vsr_engine_stats(self._e, C.byref(st))
