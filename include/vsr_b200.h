@@ -169,6 +169,14 @@ typedef struct VsrRunOpts {
     const char* checkpoint_path;
     const char* recover_path;
     double checkpoint_seconds;
+    /* seen-set host tier (delayed duplicate detection): at a level boundary where the HBM seen-set's resident entries pass a
+       load threshold, the entries of levels older than the current frontier move, unchanged, to an append-only array of up
+       to this many 16-byte entries in pinned host memory, and the table is rebuilt from the rest.  A successor equal to a
+       moved state is first inserted as new; after the level, one pass streams the tier against the table and the level's
+       rows are compacted, so totals, levels, traces and verdicts are those of a run with the whole seen-set in HBM.  Each
+       rank has its own tier.  0 = off: the seen-set is the HBM table alone.  Refused (151) together with checkpoint_path /
+       recover_path: the tier is not part of a checkpoint. */
+    uint64_t table_host_capacity;
     /* action coverage: NULL = off (the kernels are launched without the counters).  Else the BFS counts, and
        vsr_bfs_sharded (vsr_bfs, vsr_bfs_multi) writes the job's totals here when it returns, however the run ended; an
        engine created with it set counts in the stepwise interface too (vsr_engine_coverage).  Refused (151) together
@@ -203,6 +211,10 @@ typedef struct VsrStats {
     double seconds_insert;                /* several GPUs: part of seconds_kernels spent in drain-only launches */
     int32_t levels_expanded;              /* frontiers expanded = valid entries of level_generated / level_ms */
     int32_t trace_loop;                   /* rc 13: the lasso's "Back to state K" (1-based; 0 = it ends in stuttering) */
+    /* seen-set host tier (table_host_capacity > 0; summed over the ranks, times of the slowest rank per level) */
+    uint64_t host_entries;                /* seen-set entries moved to pinned host memory (each moves once, at one boundary) */
+    uint64_t host_false_new;              /* states first inserted as new that the tier pass found in host memory, removed */
+    double seconds_host_pass, seconds_host_compact, seconds_host_evict; /* tier passes, level compactions, evictions */
 } VsrStats;
 
 typedef struct VsrEngine VsrEngine;
@@ -248,6 +260,11 @@ typedef struct VsrLevelInfo {
     double ms;        /* kernel time of the level on this rank (expand + insert), CUDA events on the launch stream */
     double ms_insert; /* of which launches that only inserted records received from peers */
     int32_t violation_mask, _pad; /* OR over the level's new states of the INVARIANT bits each violates (vsr_invariant) */
+    /* seen-set host tier (table_host_capacity > 0): entries held after this boundary, this level's states removed because
+       the tier already held them (new_states excludes them), entries moved at this boundary, and the host clock of the
+       tier pass, the level's compaction and the eviction (each ends in a stream synchronise) */
+    uint64_t host_entries, false_new, evicted;
+    double ms_host_pass, ms_host_compact, ms_host_evict;
 } VsrLevelInfo;
 int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out);
 uint64_t vsr_engine_frontier_size(const VsrEngine* e);
@@ -257,7 +274,7 @@ int vsr_engine_read_frontier(VsrEngine* e, uint64_t first, uint64_t n, void* hos
 int vsr_engine_trace_record(VsrEngine* e, uint64_t local_id, uint64_t* parent_out, uint32_t* cand_out);
 int vsr_engine_stats(const VsrEngine* e, VsrStats* out);
 /* membership query: *level_out = BFS depth at which `state` (a canonical packed state) was first seen, 0 if it is not
- * in this rank's shard of the seen-set; *owner_out = the rank owning its fingerprint */
+ * in this rank's shard of the seen-set (the HBM table, then the host tier); *owner_out = the rank owning its fingerprint */
 int vsr_engine_lookup(VsrEngine* e, const void* state, int* level_out, int* owner_out);
 /* Checkpoint of this rank's shard at a level boundary (after vsr_engine_finish_level, before the next expansion): the
  * current frontier, every seen-set entry {fingerprint, meta}, the trace records and the run's statistics, to one file.

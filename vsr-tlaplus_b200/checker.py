@@ -107,7 +107,7 @@ class VsrRunOpts(C.Structure):
         ("table_capacity", C.c_uint64), ("frontier_capacity", C.c_uint64), ("max_states", C.c_uint64),
         ("max_seconds", C.c_double), ("collect_levels", C.c_int32), ("_reserved0", C.c_int32),
         ("frontier_host_capacity", C.c_uint64), ("checkpoint_path", C.c_char_p), ("recover_path", C.c_char_p),
-        ("checkpoint_seconds", C.c_double), ("coverage", C.POINTER(VsrCoverage)),
+        ("checkpoint_seconds", C.c_double), ("table_host_capacity", C.c_uint64), ("coverage", C.POINTER(VsrCoverage)),
     ]
 
 
@@ -125,6 +125,8 @@ class VsrStats(C.Structure):
         ("bytes_h2d", C.c_uint64), ("bytes_d2h", C.c_uint64), ("seconds_setup", C.c_double),
         ("records_sent", C.c_uint64), ("records_received", C.c_uint64), ("seconds_insert", C.c_double),
         ("levels_expanded", C.c_int32), ("trace_loop", C.c_int32),
+        ("host_entries", C.c_uint64), ("host_false_new", C.c_uint64),
+        ("seconds_host_pass", C.c_double), ("seconds_host_compact", C.c_double), ("seconds_host_evict", C.c_double),
     ]
 
 
@@ -158,6 +160,8 @@ class VsrLevelInfo(C.Structure):
         ("collisions", C.c_uint64), ("violation", C.c_int32), ("deadlock", C.c_int32), ("error_code", C.c_int32),
         ("overflow", C.c_int32), ("violation_id", C.c_uint64), ("deadlock_id", C.c_uint64), ("ms", C.c_double),
         ("ms_insert", C.c_double), ("violation_mask", C.c_int32), ("_pad", C.c_int32),
+        ("host_entries", C.c_uint64), ("false_new", C.c_uint64), ("evicted", C.c_uint64),
+        ("ms_host_pass", C.c_double), ("ms_host_compact", C.c_double), ("ms_host_evict", C.c_double),
     ]
 
 
@@ -367,6 +371,11 @@ class CheckResult:
     liveness: dict = field(default_factory=dict)
     trace_loop: int = 0
     coverage: Optional[Coverage] = None  # check(coverage=True): TLC's action coverage; None when it was not asked for
+    # table_host_capacity > 0: seen-set entries that ended in pinned host memory, states the tier pass removed from their
+    # level (found there after their insert), and the tier's time by part (slowest rank per level)
+    host_entries: int = 0
+    host_false_new: int = 0
+    seconds_host: dict = field(default_factory=dict)
 
     @property
     def violated(self) -> bool:
@@ -547,10 +556,12 @@ class ModelChecker:
                  frontier_capacity: int = 0, keep_trace: bool = True, collect_levels: bool = False, max_states: int = 0,
                  max_seconds: float = 0.0, stop_on_violation: bool = True, verbose: bool = False,
                  frontier_host_capacity: int = 0, checkpoint_path: Optional[str] = None, recover_path: Optional[str] = None,
-                 checkpoint_seconds: float = 0.0, coverage: bool = False) -> VsrRunOpts:
+                 checkpoint_seconds: float = 0.0, coverage: bool = False, table_host_capacity: int = 0) -> VsrRunOpts:
         """checkpoint_path / recover_path / checkpoint_seconds: TLC's -checkpoint / -recover (a file per rank at level
         boundaries; see include/vsr_b200.h VsrRunOpts).  recover_path may have been written by any number of GPUs: check()
-        and check_multi() load each rank's share of it.  coverage: count TLC's action coverage (CheckResult.coverage)"""
+        and check_multi() load each rank's share of it.  coverage: count TLC's action coverage (CheckResult.coverage).
+        table_host_capacity: seen-set entries of older levels that may move to pinned host memory, per GPU (vsrmc -tablehost;
+        not with checkpoint_path / recover_path)"""
         o = VsrRunOpts()
         if coverage:
             o.cov = VsrCoverage()  # kept alive by the options object
@@ -572,6 +583,7 @@ class ModelChecker:
         o.checkpoint_path = checkpoint_path.encode() if checkpoint_path else None
         o.recover_path = recover_path.encode() if recover_path else None
         o.checkpoint_seconds = checkpoint_seconds
+        o.table_host_capacity = table_host_capacity
         return o
 
     def result_from_stats(self, st: VsrStats, rc: int, trace=None, levels=None) -> CheckResult:
@@ -588,7 +600,8 @@ class ModelChecker:
             bytes_d2h=int(st.bytes_d2h), seconds_setup=float(st.seconds_setup),
             violated_invariants=[name] if name else [],
             records_sent=int(st.records_sent), records_received=int(st.records_received), seconds_insert=float(st.seconds_insert),
-            trace=trace or [], levels=levels or [])
+            trace=trace or [], levels=levels or [], host_entries=int(st.host_entries), host_false_new=int(st.host_false_new),
+            seconds_host={"pass": float(st.seconds_host_pass), "compact": float(st.seconds_host_compact), "evict": float(st.seconds_host_evict)})
 
     @staticmethod
     def _coverage_of(o: VsrRunOpts) -> Optional[Coverage]:

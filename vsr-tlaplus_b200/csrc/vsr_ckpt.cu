@@ -28,6 +28,7 @@ using namespace vsr;
 namespace {
 
 constexpr uint64_t CKPT_MAGIC = 0x3154504B43525356ull; /* "VSRCKPT1" */
+constexpr uint32_t CKPT_VERSION = 2; /* 2: VsrStats ends with the seen-set host tier's figures */
 
 struct CkptHeader {
     uint64_t magic;
@@ -41,48 +42,6 @@ struct CkptHeader {
     uint64_t n_trace;                     /* trace records that follow (0 without keep_trace) */
     uint64_t records_sent, records_received;
 };
-
-/* non-empty entries of table slots [first, first + n) appended to out[] (order is irrelevant); one atomic per warp */
-__global__ void ckpt_compact_kernel(const uint64_t* __restrict__ table, unsigned long long first, unsigned long long n, uint64_t* __restrict__ out,
-                                    unsigned long long* count) {
-    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
-    const unsigned long long rounds = (n + stride - 1) / stride;
-    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int lane = threadIdx.x & 31;
-    for (unsigned long long r = 0; r < rounds; r++, i += stride) { /* whole warps stay in the loop: the ballot below is warp-wide */
-        uint64_t e0 = 0, e1 = 0;
-        if (i < n) {
-            e0 = table[2 * (first + i)];
-            e1 = table[2 * (first + i) + 1];
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, e0 != 0);
-        if (!m) continue;
-        unsigned long long base = 0;
-        const int leader = __ffs(m) - 1;
-        if (lane == leader) base = atomicAdd(count, (unsigned long long)__popc(m));
-        base = __shfl_sync(0xffffffffu, base, leader);
-        if (e0) {
-            const unsigned long long pos = base + __popc(m & ((1u << lane) - 1u));
-            out[2 * pos] = e0;
-            out[2 * pos + 1] = e1;
-        }
-    }
-}
-
-/* entries of a checkpoint back into a (fresh) table: every one must be new.  owner_shift < 64 (a checkpoint of another
-   number of ranks): only the entries this rank owns, counted in *owned; 64 inserts every entry */
-__global__ void ckpt_reinsert_kernel(uint64_t* table, unsigned long long cap, const uint64_t* __restrict__ ents, unsigned long long n,
-                                     int owner_shift, int rank, unsigned long long* not_new, unsigned long long* owned) {
-    unsigned long long bad = 0, mine = 0;
-    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
-        if (owner_shift < 64 && owner_of(ents[2 * i], owner_shift) != rank) continue;
-        unsigned probes = 0, coll = 0;
-        mine++;
-        if (table_insert(table, cap, ents[2 * i], ents[2 * i + 1], probes, coll) != INS_NEW) bad++;
-    }
-    if (bad) atomicAdd(not_new, bad);
-    if (owned && mine) atomicAdd(owned, mine);
-}
 
 /* old trace records renumbered into the new world's ids */
 __global__ void ckpt_remap_trace_kernel(const uint64_t* __restrict__ in, unsigned long long n, const SpillRows out, const GidRemap m) {
@@ -103,7 +62,7 @@ int io_error(VsrEngine* e, const char* what, const char* path) {
 constexpr uint64_t IO_CHUNK = 64ull << 20; /* bytes per host staging round */
 
 bool header_ok(const CkptHeader& h) {
-    return h.magic == CKPT_MAGIC && h.version == 1 && h.header_bytes == sizeof h && h.stats_bytes == sizeof(VsrStats);
+    return h.magic == CKPT_MAGIC && h.version == CKPT_VERSION && h.header_bytes == sizeof h && h.stats_bytes == sizeof(VsrStats);
 }
 
 /* 1: a checkpoint header of this build, 0: something else, -1: the file cannot be opened */
@@ -124,12 +83,19 @@ int seek(VsrEngine* e, File& f, uint64_t at, const char* path) {
     return 0;
 }
 
+/* the host tier holds seen-set entries a checkpoint file has no section for */
+int refuse_host_tier(VsrEngine* e) {
+    snprintf(e->last_error, sizeof e->last_error, "%s", HOST_TIER_NO_CHECKPOINT);
+    return VSR_RC_CONFIG_ERROR;
+}
+
 } // namespace
 
 extern "C" {
 
 int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals) {
     if (!e || !path) return VSR_RC_ERROR;
+    if (e->seen_host.host_rows) return refuse_host_tier(e);
     if (e->level_open) {
         snprintf(e->last_error, sizeof e->last_error, "checkpoint: only at a level boundary (after vsr_engine_finish_level)");
         return VSR_RC_ERROR;
@@ -144,7 +110,7 @@ int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals
     CkptHeader h;
     memset(&h, 0, sizeof h);
     h.magic = CKPT_MAGIC;
-    h.version = 1;
+    h.version = CKPT_VERSION;
     h.header_bytes = sizeof h;
     h.stats_bytes = sizeof(VsrStats);
     h.state_bytes = (uint32_t)S;
@@ -180,7 +146,7 @@ int vsr_engine_checkpoint(VsrEngine* e, const char* path, const VsrStats* totals
         for (uint64_t first = 0; first < e->table_cap; first += slots_per_pass) {
             const uint64_t n = std::min(slots_per_pass, e->table_cap - first);
             CK(cudaMemsetAsync(dcount, 0, 8, e->stream));
-            ckpt_compact_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, first, n, scratch, dcount);
+            seen_compact_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, first, n, 0, 256, SpillRows{(uint32_t*)scratch, nullptr, ~0ull}, ~0ull, dcount);
             CK(cudaGetLastError());
             unsigned long long cnt = 0;
             CK(cudaMemcpyAsync(&cnt, dcount, 8, cudaMemcpyDeviceToHost, e->stream));
@@ -264,6 +230,7 @@ int old_files(VsrEngine* e, const char* base, std::vector<std::string>& files) {
 
 extern "C" int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* totals_out) {
     if (!e || !path) return VSR_RC_ERROR;
+    if (e->seen_host.host_rows) return refuse_host_tier(e);
     CK(cudaSetDevice(e->device));
     std::vector<std::string> files;
     int rc = old_files(e, path, files);
@@ -377,7 +344,7 @@ extern "C" int vsr_engine_recover(VsrEngine* e, const char* path, VsrStats* tota
                 t_read += now_s() - t;
                 t = now_s();
                 CK(cudaMemcpyAsync(scratch, host.data(), n * 16, cudaMemcpyHostToDevice, e->stream));
-                ckpt_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, (const uint64_t*)scratch, n, e->owner_shift, me, d0, d1);
+                seen_reinsert_kernel<<<e->sms * 8, 256, 0, e->stream>>>(e->table, e->table_cap, SpillRows{(uint32_t*)scratch, nullptr, ~0ull}, n, e->owner_shift, me, d0, d1);
                 CK(cudaGetLastError());
                 CK(cudaMemcpyAsync(counts, d0, 16, cudaMemcpyDeviceToHost, e->stream));
                 CK(cudaStreamSynchronize(e->stream)); /* `host` is reused by the next round */

@@ -83,6 +83,15 @@ struct VsrEngine {
     vsr::LiveCtr* live_ctr = nullptr;
     std::vector<uint64_t> live_level_off; /* live_level_off[d - 1] = store index of depth d's first state; back() = stored */
     uint64_t live_bytes_hbm = 0, live_bytes_host = 0;
+    /* seen-set host tier (opts.table_host_capacity > 0; vsr_seen_host.cu): entries {fp, meta} of levels below evict_floor,
+       appended at level boundaries to rows of 4 words in pinned host memory.  table_resident = entries in the HBM table.
+       Table entries tagged below evict_floor are states the tier already holds (marked by a tier pass): the next eviction
+       drops them instead of appending them again */
+    vsr::SpillBuffer seen_host;
+    uint64_t seen_host_n = 0;
+    uint64_t table_resident = 0;
+    int evict_floor = 0;
+    unsigned long long* seen_host_ctr = nullptr; /* 4 device counters of the tier's kernels */
     char last_error[256] = {0};
 };
 
@@ -96,6 +105,15 @@ int live_create(VsrEngine* e, char* err, size_t errcap);
 void live_destroy(VsrEngine* e);
 int live_reset(VsrEngine* e);
 int live_collect(VsrEngine* e);
+/* vsr_seen_host.cu: the host tier's allocation and release; the tier pass and the compaction of the level just generated
+   (finish_level, after the VIEW-tie patch, before anything reads the level: lc is read again, li gets the tier's figures);
+   the eviction at the boundary that follows; the tier's part of a membership query (the level, 0 if absent) */
+cudaError_t seen_host_create(VsrEngine* e);
+void seen_host_destroy(VsrEngine* e);
+int seen_host_filter(VsrEngine* e, vsr::LevelCounters& lc, size_t ctr_bytes, VsrLevelInfo& li);
+int seen_host_evict(VsrEngine* e, VsrLevelInfo& li);
+int seen_host_lookup(const VsrEngine* e, uint64_t fp, uint32_t check);
+#define HOST_TIER_NO_CHECKPOINT "-checkpoint / -recover with a seen-set host tier (-tablehost, table_host_capacity > 0): the host tier is not part of a checkpoint"
 /* vsr_shard.cu: the candidate chain from Init to global state id `gid` (every rank of a group calls it together) */
 int walk_trace(VsrEngine* e, uint64_t gid, std::vector<uint32_t>& cands);
 

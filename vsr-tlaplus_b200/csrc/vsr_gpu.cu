@@ -157,6 +157,9 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
         return fail(VSR_RC_CONFIG_ERROR, "world must be 1, 2, 4 or 8 and 0 <= rank < world");
     if (m->info.property && world > 1)
         return fail(VSR_RC_CONFIG_ERROR, "PROPERTY ViewChangeCompletes is checked on one GPU only: liveness on several GPUs is not supported");
+    if (opts->table_host_capacity && opts->coverage && !opts->keep_trace)
+        return fail(VSR_RC_CONFIG_ERROR, "coverage with a seen-set host tier needs the trace (keep_trace): a state the tier pass removes gives its "
+                                         "distinct count back to the action of its trace record");
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
     if (ce != cudaSuccess || ndev == 0)
@@ -208,7 +211,8 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     if (!fcap) fcap = (uint64_t)(free_b * (live ? 0.15 : 0.40)) / (2 * S);
     if (fcap < 64) fcap = 64;
     e->table_cap = tcap;
-    e->trace_cap = opts->keep_trace ? tcap - tcap / 8 + 64 : 0; /* one record per distinct state, up to the seen-set's load limit */
+    /* one record per distinct state, up to the seen-set's load limit and what its host tier holds */
+    e->trace_cap = opts->keep_trace ? tcap - tcap / 8 + 64 + opts->table_host_capacity : 0;
     e->tie_cap = 1 << 16;
     if ((ce = cudaMallocAsync((void**)&e->table, tcap * 16, e->stream)) != cudaSuccess) return bail("cudaMalloc(seen-set)", ce);
     if ((ce = cudaMemsetAsync(e->table, 0, tcap * 16, e->stream)) != cudaSuccess) return bail("memset", ce);
@@ -222,6 +226,7 @@ int vsr_engine_create(const VsrModel* m, const VsrRunOpts* opts, int rank, int w
     if ((ce = cudaMallocAsync((void**)&e->init_rec, e->g->rec_bytes, e->stream)) != cudaSuccess) return bail("cudaMalloc", ce);
     if ((ce = cudaMemcpyAsync(e->fp_tab, fp64_table(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream)) != cudaSuccess) return bail("memcpy", ce);
     if ((ce = trace_alloc(e)) != cudaSuccess) return bail(e->trace.host_rows ? "cudaHostAlloc(trace)" : "cudaMalloc(trace)", ce);
+    if ((ce = seen_host_create(e)) != cudaSuccess) return bail("cudaHostAlloc(seen-set host tier)", ce);
     e->st.table_capacity = tcap;
     e->st.frontier_capacity = e->frontier[0].capacity();
     e->st.bytes_table = tcap * 16;
@@ -249,6 +254,7 @@ void vsr_engine_destroy(VsrEngine* e) {
     if (e->stream) cudaFreeAsync(e->fp_tab, e->stream); else cudaFree(e->fp_tab);
     if (e->stream) cudaFreeAsync(e->init_rec, e->stream); else cudaFree(e->init_rec);
     live_destroy(e);
+    seen_host_destroy(e);
     vsr_engine_detach(e);
     delete e->cov;
     if (e->ev0) cudaEventDestroy(e->ev0);
@@ -407,6 +413,11 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
     }
     VsrLevelInfo li;
     memset(&li, 0, sizeof li);
+    const uint64_t hbm_new = c.out_count; /* inserted into the HBM table as new this level, false new states included */
+    if (e->seen_host_n && !c.overflow && c.out_count && c.out_count <= fcap_total) {
+        const int rc = seen_host_filter(e, lc, ctr_bytes, li);
+        if (rc) return rc;
+    }
     li.new_states = c.out_count;
     li.generated = c.generated;
     li.frontier_in = e->n_cur;
@@ -435,7 +446,17 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
                  c.overflow == 1 ? "frontier" : (c.overflow == 2 ? "tie list" : (c.overflow == 3 ? "send buffer" : "seen-set")), (unsigned long long)c.out_count,
                  (unsigned long long)fcap_total);
     }
-    if (!li.overflow && e->st.distinct + c.out_count > e->table_cap - e->table_cap / 8) {
+    if (e->seen_host.host_rows) { /* the table holds what the last eviction kept and every level inserted since */
+        if (!li.overflow && e->table_resident + hbm_new > e->table_cap - e->table_cap / 8) {
+            li.overflow = 4;
+            snprintf(e->last_error, sizeof e->last_error,
+                     "capacity exceeded (seen-set): %llu entries in HBM with this level's %llu new states (false ones included) in %llu slots; "
+                     "the host tier holds %llu of %llu entries",
+                     (unsigned long long)(e->table_resident + hbm_new), (unsigned long long)hbm_new, (unsigned long long)e->table_cap,
+                     (unsigned long long)e->seen_host_n, (unsigned long long)e->seen_host.host_rows);
+        }
+        e->table_resident += hbm_new;
+    } else if (!li.overflow && e->st.distinct + c.out_count > e->table_cap - e->table_cap / 8) {
         li.overflow = 4; /* seen-set load above 7/8: probe chains explode long before it is literally full */
         snprintf(e->last_error, sizeof e->last_error, "capacity exceeded (seen-set): %llu distinct states in %llu slots",
                  (unsigned long long)(e->st.distinct + c.out_count), (unsigned long long)e->table_cap);
@@ -491,6 +512,11 @@ int vsr_engine_finish_level(VsrEngine* e, VsrLevelInfo* out) {
         if (n_new && vsr_engine_read_frontier(e, 0, n_new, host.data())) return VSR_RC_SYSTEM;
         e->collected.push_back(std::move(host));
     }
+    if (e->seen_host.host_rows && !li.overflow) { /* the boundary: nothing is in flight, the next level is not open */
+        const int rc = seen_host_evict(e, li);
+        if (rc && rc != VSR_RC_TOO_LARGE) return rc;
+        li.host_entries = e->seen_host_n;
+    }
     if (out) *out = li;
     return 0;
 }
@@ -529,6 +555,7 @@ int vsr_engine_lookup(VsrEngine* e, const void* state, int* level_out, int* owne
     CK(cudaMemcpyAsync(&meta, d, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     *level_out = (int)(meta >> 56);
+    if (!meta && e->seen_host_n) *level_out = seen_host_lookup(e, fp, chk);
     return 0;
 }
 
@@ -578,6 +605,7 @@ int vsr_engine_reset(VsrEngine* e) {
     e->st.table_capacity = tc; e->st.frontier_capacity = fc; e->st.bytes_table = bt; e->st.bytes_frontier = bf;
     e->cur = 0; e->n_cur = 0; e->cur_base = 0; e->next_base = 0; e->level = 0; e->level_open = false;
     e->records_sent = e->records_received = 0;
+    e->seen_host_n = 0; e->table_resident = 0; e->evict_floor = 0;
     e->collected.clear();
     if (e->cov) memset(e->cov, 0, sizeof *e->cov);
     return live_reset(e);
@@ -742,6 +770,7 @@ int vsr_probe_bench(int device, uint64_t capacity, uint64_t n, double dup_frac, 
 
 } /* extern "C" */
 
-/* the liveness pass is part of this translation unit: the library's sources stay the four the single-layout builds of
-   the tests and tools compile (vsr_gpu.cu, vsr_shard.cu, vsr_ckpt.cu, vsr_host.cpp) */
+/* the liveness pass and the seen-set's host tier are part of this translation unit: the library's sources stay the four
+   the single-layout builds of the tests and tools compile (vsr_gpu.cu, vsr_shard.cu, vsr_ckpt.cu, vsr_host.cpp) */
 #include "vsr_live.cu"
+#include "vsr_seen_host.cu"

@@ -7,6 +7,7 @@
 
 #include "vsr_gpu.cuh"
 #include "vsr_live.cuh"
+#include "vsr_seen_host.cuh"
 #include "vsr_model.h"
 
 namespace vsr {
@@ -29,12 +30,14 @@ struct GpuOps {
     cudaError_t (*launch_live_sweep)(const LiveParams&, int sms, cudaStream_t);
     /* recovery on another number of ranks (vsr_ckpt.cu): keep this rank's share of one chunk of an old rank's frontier */
     cudaError_t (*launch_reshard_frontier)(const ReshardParams&, int sms, cudaStream_t);
+    /* seen-set host tier (vsr_seen_host.cuh): one phase of a level's compaction */
+    cudaError_t (*launch_seen_host_compact)(const SeenHostParams&, int sms, cudaStream_t);
 };
 
 /* what a layout plug-in must have been compiled against: the version constant AND the shapes of the structs the kernels and the
    host exchange (a plug-in built from another revision of these headers must be rebuilt, never loaded) */
 inline int gpu_abi_value() {
-    return VSR_PLUGIN_ABI * 100000 + (int)((sizeof(ExpandParams) * 131 + sizeof(LiveParams) * 61 + sizeof(ReshardParams) * 29 + sizeof(DevCounters) * 17 +
+    return VSR_PLUGIN_ABI * 100000 + (int)((sizeof(ExpandParams) * 131 + sizeof(LiveParams) * 61 + sizeof(ReshardParams) * 29 + sizeof(SeenHostParams) * 7 + sizeof(DevCounters) * 17 +
                                             sizeof(SpillRows) * 5 + sizeof(RecHdr) + VSR_BUCKET * 3) % 100000);
 }
 
@@ -91,13 +94,20 @@ template <class L> struct GpuThunks {
         reshard_frontier_kernel<L><<<(unsigned)(want < most ? want : most), 256, 0, st>>>(q);
         return cudaGetLastError();
     }
+    static cudaError_t launch_seen_host_compact(const SeenHostParams& q, int sms, cudaStream_t st) {
+        const unsigned long long n = q.phase ? q.n - q.n_keep : q.n_keep;
+        if (!n) return cudaSuccess;
+        const unsigned long long want = (n + 255) / 256, most = (unsigned long long)sms * 8;
+        seen_host_compact_kernel<L><<<(unsigned)(want < most ? want : most), 256, 0, st>>>(q);
+        return cudaGetLastError();
+    }
     static uint32_t chk(const uint32_t* w, int use_view) { return check_hash<L>(w, use_view != 0); }
     static const GpuOps* get() {
         typedef ExpandCfg<L> Cfg;
         static const GpuOps ops = {chk, L::R, L::V, L::K, L::NW, L::BYTES, (int)(L::BYTES + sizeof(RecHdr)), sizeof(typename Cfg::Smem), Cfg::WARPS * 32,
                                    launch_expand, launch_patch, (int)(sizeof(TieRec) + L::BYTES), prepare, launch_simulate,
                                    Cfg::WARPS, Cfg::BLOCKS, Cfg::PASSES, Expander<L, false>::SROWS, launch_audit,
-                                   launch_live_collect, launch_live_sweep, launch_reshard_frontier};
+                                   launch_live_collect, launch_live_sweep, launch_reshard_frontier, launch_seen_host_compact};
         return &ops;
     }
 };

@@ -59,7 +59,7 @@ uint64_t live_stored(const VsrEngine* e) { return e->live_level_off.empty() ? 0 
 
 } // namespace
 
-/* Sizes, up front: the store holds as many states as the seen-set (its load limit), unless VSR_B200_LIVE_STATES says fewer;
+/* Sizes, up front: the store holds as many states as the seen-set (its load limit, plus its host tier), unless VSR_B200_LIVE_STATES says fewer;
    the live index has two slots per stored state (load <= 1/2), the local ids 8 B and the alive bits 1 bit per state in HBM.
    The words go to HBM as far as it has room (VSR_B200_LIVE_HBM_STATES caps that part, for tests) and continue in pinned host
    memory mapped into the device when the run allows host memory (frontier_host_capacity > 0, as for the frontier spill);
@@ -70,7 +70,7 @@ int live_create(VsrEngine* e, char* err, size_t errcap) {
         return rc;
     };
     const uint64_t S = (uint64_t)e->g->bytes;
-    uint64_t cap = e->table_cap - e->table_cap / 8;
+    uint64_t cap = e->table_cap - e->table_cap / 8 + e->opts.table_host_capacity; /* the seen-set with its host tier */
     if (const uint64_t want = env_u64("VSR_B200_LIVE_STATES")) cap = std::min(cap, want);
     cap = std::min<uint64_t>(cap, 0xFFFFFFFEull); /* the index's meta carries store index + 1 in 32 bits */
     cap = (cap + 31) & ~31ull;

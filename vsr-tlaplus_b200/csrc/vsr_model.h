@@ -52,7 +52,7 @@ struct ModelOps {
     int (*property)(const RunCfg*, const uint32_t*, int live_hooks);   /* the liveness pass's state predicate (live_pred) */
 };
 /* bump when ModelOps / GpuOps / ExpandParams / LiveParams / ReshardParams / SimParams change shape: a layout plug-in built against another value is rebuilt */
-#define VSR_PLUGIN_ABI 13
+#define VSR_PLUGIN_ABI 14
 const ModelOps* find_model_ops(int R, int V, int K);
 const GpuOps* find_gpu_ops(int R, int V, int K); /* defined in vsr_gpu.cu */
 

@@ -49,6 +49,8 @@ struct StepMsg {
 struct LevelMsg {
     uint64_t new_states, generated, ties, collisions, frontier, viol_id, dead_id, sent, received;
     double ms, ms_insert;
+    uint64_t host_entries, false_new;                 /* the seen-set's host tier */
+    double ms_host_pass, ms_host_compact, ms_host_evict;
     int32_t violation, deadlock, error_code, overflow, late, failed, ckpt, _pad;
 };
 static_assert(sizeof(LevelMsg) <= VSR_GROUP_MSG_BYTES, "all-gather slot");
@@ -251,6 +253,10 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
     engine_set_coverage(e, opts->coverage != nullptr);
     std::vector<VsrCoverage> cov(opts->coverage ? 1 : 0); /* the job's totals (the engine's own are this rank's) */
     if (opts->coverage) memset(&cov[0], 0, sizeof cov[0]);
+    if (opts->table_host_capacity && (opts->checkpoint_path || opts->recover_path)) {
+        snprintf(e->last_error, sizeof e->last_error, "%s", HOST_TIER_NO_CHECKPOINT);
+        return VSR_RC_CONFIG_ERROR;
+    }
     if (e->m->info.property && (opts->checkpoint_path || opts->recover_path)) {
         snprintf(e->last_error, sizeof e->last_error, "-checkpoint / -recover with PROPERTY ViewChangeCompletes: checkpointing the liveness store is not supported");
         return VSR_RC_CONFIG_ERROR;
@@ -325,6 +331,8 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
         mine.viol_id = li.violation ? make_gid(me, li.violation_id) : ~0ull;
         mine.dead_id = li.deadlock ? make_gid(me, li.deadlock_id) : ~0ull;
         mine.ms = li.ms; mine.ms_insert = li.ms_insert;
+        mine.host_entries = e->seen_host_n; mine.false_new = li.false_new;
+        mine.ms_host_pass = li.ms_host_pass; mine.ms_host_compact = li.ms_host_compact; mine.ms_host_evict = li.ms_host_evict;
         mine.late = opts->max_seconds > 0 && now_s() - t0 >= opts->max_seconds;
         mine.ckpt = !ckpt_path.empty() && now_s() - last_ckpt >= opts->checkpoint_seconds;
         if (W > 1) {
@@ -332,8 +340,12 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
         } else all[0] = mine;
         uint64_t n_new = 0, n_gen = 0, max_frontier = 0, vmin = ~0ull, dmin = ~0ull;
         int viol = 0, dead = 0, err = 0, ovf = 0, failed = 0;
-        double ms = 0, msi = 0;
+        double ms = 0, msi = 0, ms_pass = 0, ms_compact = 0, ms_evict = 0;
+        uint64_t host_entries = 0, false_new = 0;
         for (int r = 0; r < W; r++) {
+            host_entries += all[r].host_entries; false_new += all[r].false_new;
+            ms_pass = std::max(ms_pass, all[r].ms_host_pass); ms_compact = std::max(ms_compact, all[r].ms_host_compact);
+            ms_evict = std::max(ms_evict, all[r].ms_host_evict);
             n_new += all[r].new_states; n_gen += all[r].generated;
             tot.h2_ties += all[r].ties; tot.fp_collisions += all[r].collisions;
             max_frontier = std::max(max_frontier, all[r].frontier);
@@ -372,6 +384,11 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
         insert_ms += msi;
         tot.generated += n_gen;
         tot.distinct += n_new;
+        tot.host_entries = host_entries;
+        tot.host_false_new += false_new;
+        tot.seconds_host_pass += ms_pass * 1e-3;
+        tot.seconds_host_compact += ms_compact * 1e-3;
+        tot.seconds_host_evict += ms_evict * 1e-3;
         const bool boundary_only = resumed; /* first pass after a recovery: stands at the checkpoint's level boundary */
         if (resumed) { /* the totals, level tables and verdicts up to this boundary came with the checkpoint */
             resumed = false;
@@ -385,7 +402,11 @@ int vsr_bfs_sharded(VsrEngine* e, const VsrRunOpts* opts, uint64_t part_states, 
             tot.num_levels = level;
         }
         if (opts->verbose && me == 0 && level >= 2 && !boundary_only)
-            fprintf(stderr, "depth %3d: %12llu new  %12llu generated  %8.3f ms%s\n", level, (unsigned long long)n_new, (unsigned long long)n_gen, ms, slowest.c_str());
+            fprintf(stderr, "depth %3d: %12llu new  %12llu generated  %8.3f ms%s", level, (unsigned long long)n_new, (unsigned long long)n_gen, ms, slowest.c_str());
+        if (opts->verbose && me == 0 && level >= 2 && !boundary_only && opts->table_host_capacity)
+            fprintf(stderr, "  host tier %llu entries, %llu false new removed, pass %.3f ms, compaction %.3f ms, eviction %.3f ms", (unsigned long long)host_entries,
+                    (unsigned long long)false_new, ms_pass, ms_compact, ms_evict);
+        if (opts->verbose && me == 0 && level >= 2 && !boundary_only) fprintf(stderr, "\n");
         if (err) { result = VSR_RC_ERROR; tot.error_code = err; break; }
         if (ovf) { result = VSR_RC_TOO_LARGE; break; }
         if (viol && !tot.violation_level) {

@@ -79,6 +79,9 @@ struct SpillBuffer {
     }
     uint64_t capacity() const { return hbm_rows + host_rows; }
     SpillRows view() const { return {hbm, host, host_rows ? hbm_rows : ~0ull}; }
+    /* the same memory as rows of `words` 4-byte words (scratch space for another kind of row), and how many fit */
+    SpillRows view_as(int words) const { return {hbm, host, host_rows ? hbm_rows * row_bytes / (4 * words) : ~0ull}; }
+    uint64_t capacity_as(int words) const { return (hbm_rows * row_bytes) / (4 * words) + (host_rows * row_bytes) / (4 * words); }
     /* rows [first, first + n) <-> host memory: the HBM part by cudaMemcpy, the host part directly */
     cudaError_t to_host(uint64_t first, uint64_t n, void* dst) const {
         const uint64_t k = first < hbm_rows ? (n < hbm_rows - first ? n : hbm_rows - first) : 0;

@@ -117,6 +117,8 @@ class ShardedResult:
     trace_cands: List[int] = field(default_factory=list)
     trace: List[Tuple[str, bytes]] = field(default_factory=list)
     coverage: Optional["ck.Coverage"] = None  # GpuEngine(coverage=True): the job's action coverage (the same on every rank)
+    host_entries: int = 0            # table_host_capacity > 0: seen-set entries in host memory (all ranks), states removed
+    host_false_new: int = 0
     # check_sharded only: this rank's wall clock of the one-call API by part (engine creation = allocation + clearing the
     # seen-set; attach = inbox allocation + CUDA IPC mapping of the peers; bfs; replay of the counterexample; teardown)
     call_seconds: dict = field(default_factory=dict)
@@ -128,7 +130,7 @@ class GpuEngine:
     def __init__(self, mc: "ck.ModelChecker", rank: int, world: int, device: int = 0, table_capacity: int = 0,
                  frontier_capacity: int = 0, inbox_records: int = 0, keep_trace: bool = True, check_deadlock: bool = False,
                  collect_levels: bool = False, group: Optional[Group] = None, exchange: str = "p2p", frontier_host_capacity: int = 0,
-                 coverage: bool = False):
+                 coverage: bool = False, table_host_capacity: int = 0):
         if coverage and world > 1 and exchange != "p2p":
             # the staged pump (ShardedBfs) sums no per-level action counts over the ranks
             raise ck.VsrError(151, "coverage with exchange='staged' is not supported: use the fused exchange (exchange='p2p')")
@@ -138,7 +140,8 @@ class GpuEngine:
         self.exchange = exchange if world > 1 else "none"
         self._opts = mc.run_opts(deadlock=check_deadlock, device=device, table_capacity=table_capacity,
                                  frontier_capacity=frontier_capacity, keep_trace=keep_trace, collect_levels=collect_levels,
-                                 frontier_host_capacity=frontier_host_capacity, coverage=coverage)
+                                 frontier_host_capacity=frontier_host_capacity, coverage=coverage,
+                                 table_host_capacity=table_host_capacity)
         self._e = C.c_void_p()
         err = C.create_string_buffer(512)
         t0 = time.time()
@@ -199,7 +202,8 @@ class GpuEngine:
                           violation_gid=int(st.violation_id) if st.violation_level else -1, seconds=float(st.seconds_total),
                           kernel_ms_max=float(st.seconds_kernels) * 1e3, insert_ms_max=float(st.seconds_insert) * 1e3,
                           exchanged_records=int(st.records_sent), received_records=int(st.records_received),
-                          launches=int(st.kernel_launches), bytes_h2d=int(st.bytes_h2d), bytes_d2h=int(st.bytes_d2h))
+                          launches=int(st.kernel_launches), bytes_h2d=int(st.bytes_h2d), bytes_d2h=int(st.bytes_d2h),
+                          host_entries=int(st.host_entries), host_false_new=int(st.host_false_new))
         if want_trace and (rc in (11, 12) or r.violation_level):
             r.trace_cands = [int(cands[i]) for i in range(int(n.value))]
         r.coverage = self.mc._coverage_of(o)
@@ -305,12 +309,13 @@ class GpuEngine:
 
 def check_sharded(mc: "ck.ModelChecker", group: Group, device: int = 0, table_capacity: int = 0, frontier_capacity: int = 0,
                   inbox_records: int = 0, part_states: int = 0, keep_trace: bool = True, check_deadlock: bool = False,
-                  coverage: bool = False, **run_kw) -> ShardedResult:
+                  coverage: bool = False, table_host_capacity: int = 0, **run_kw) -> ShardedResult:
     """One call per rank: engine + inbox + BFS + teardown; on a violation rank 0's result carries the literal trace.
     coverage: count TLC's action coverage (ShardedResult.coverage, the job's totals on every rank).  recover_path= (in
     run_kw) continues a checkpoint written by any number of ranks."""
     eng = GpuEngine(mc, group.rank, group.world, device=device, table_capacity=table_capacity, frontier_capacity=frontier_capacity,
-                    inbox_records=inbox_records, keep_trace=keep_trace, check_deadlock=check_deadlock, group=group, coverage=coverage)
+                    inbox_records=inbox_records, keep_trace=keep_trace, check_deadlock=check_deadlock, group=group, coverage=coverage,
+                    table_host_capacity=table_host_capacity)
     res = None
     try:
         t0 = time.time()
